@@ -416,7 +416,8 @@ class Stream:
         out_schema = Schema(self.schema.key, "i")
         in_tr, out_tr = Spine(be, w.schema), Spine(be, pair_schema)
         nk = self.schema.nk
-        avg = Proj(out_schema, [key(i) for i in range(nk)] + [lval(0) // lval(1)])
+        # a key whose count sums to 0 (its sum need not) has no average: no row, where the reference panics
+        avg = Proj(out_schema, [key(i) for i in range(nk)] + [lval(0) // lval(1)], where=[lval(1).ne(0)])
 
         def fn(d: Batch):
             in_tr.insert(d)

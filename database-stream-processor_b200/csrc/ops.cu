@@ -55,9 +55,11 @@ __device__ __forceinline__ u64 expr_val(const dbsp_expr& x, const E& e) {
     case DBSP_OP_ADD: return a + src_val(x.b, e);
     case DBSP_OP_SUB: return a - src_val(x.b, e);
     case DBSP_OP_MUL: return a * src_val(x.b, e);
-    case DBSP_OP_DIV: {
+    case DBSP_OP_DIV: {   // i64::wrapping_div, x / 0 = 0: MIN / -1 wraps to MIN instead of trapping
       i64 d = (i64)src_val(x.b, e);
-      return d == 0 ? 0 : (u64)((i64)a / d);
+      if (d == 0) return 0;
+      if (d == -1) return (u64)0 - a;
+      return (u64)((i64)a / d);
     }
   }
   return a;

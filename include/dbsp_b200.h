@@ -70,7 +70,10 @@ enum dbsp_src_kind {
 };
 enum dbsp_expr_op {
   DBSP_OP_COPY = 0, DBSP_OP_NEG = 1, DBSP_OP_ADD = 2, DBSP_OP_SUB = 3,
-  DBSP_OP_MUL = 4, DBSP_OP_DIV = 5 /* signed, truncating (Rust isize `/`) */
+  DBSP_OP_MUL = 4,
+  DBSP_OP_DIV = 5 /* signed, truncating (Rust isize `/`), wrapping: x / 0 = 0
+                     and MIN / -1 = MIN (i64::wrapping_div); NEG/ADD/SUB/MUL
+                     wrap mod 2^64 */
 };
 enum dbsp_cmp_op {
   DBSP_CMP_EQ = 0, DBSP_CMP_NE = 1, DBSP_CMP_LT = 2, DBSP_CMP_LE = 3,

@@ -653,7 +653,12 @@ inline u64 expr_val(const dbsp_expr& x, const Env& e) {
     case DBSP_OP_ADD: return a + src_val(x.b, e);
     case DBSP_OP_SUB: return a - src_val(x.b, e);
     case DBSP_OP_MUL: return a * src_val(x.b, e);
-    case DBSP_OP_DIV: { i64 d = (i64)src_val(x.b, e); return d == 0 ? 0 : (u64)((i64)a / d); }
+    case DBSP_OP_DIV: {   // i64::wrapping_div, x / 0 = 0 (the ABI's rules; Rust's `/` panics on both)
+      i64 d = (i64)src_val(x.b, e);
+      if (d == 0) return 0;
+      if (d == -1) return (u64)0 - a;   // MIN / -1 = MIN; the C++ division would trap
+      return (u64)((i64)a / d);
+    }
   }
   return a;
 }

@@ -281,7 +281,8 @@ struct Q4 : Query {
     pj = proj(schema("uu", "u"), {cp(K(0)), cp(LV(0)), cp(RV(0))}, {pr(DBSP_CMP_GE, RV(1), LV(1)), pr(DBSP_CMP_LE, RV(1), LV(2))});
     pcat = proj(schema("u", "u"), {cp(K(1)), cp(LV(0))});
     fw = cp(LV(0));
-    pavg = proj(schema("u", "i"), {cp(K(0)), ex(DBSP_OP_DIV, LV(0), LV(1))});
+    // a key whose count sums to 0 has no average (as Stream.average)
+    pavg = proj(schema("u", "i"), {cp(K(0)), ex(DBSP_OP_DIV, LV(0), LV(1))}, {pr(DBSP_CMP_NE, LV(1), CST(0))});
     pfin = proj(schema("uu", ""), {cp(K(0)), cp(LV(0))});
     lt = new_spine(w, pa.out_schema);
     rt = new_spine(w, pb.out_schema);

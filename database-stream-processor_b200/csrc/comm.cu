@@ -16,6 +16,7 @@
 //     only after the kernels that consume round s were queued before it on its stream, and a rank writes round s+2
 //     only after it saw every peer's signal of round s+1 — so the flags themselves order slot reuse; no extra ack.
 //   * All replicas issue the same sequence of exchange calls (SPMD, like the reference's workers).
+#include <cuda.h>
 #include <unistd.h>
 
 #include "ops.cuh"
@@ -316,6 +317,21 @@ int32_t comm_create(Ctx* ctx, int rank, int world, u64 slot_bytes, unsigned char
   return DBSP_OK;
 }
 
+// CUDA's lazy loading (the default since CUDA 12.2) loads a kernel at its first launch, and the load waits for the
+// kernels running in the same CUDA context.  Ranks that share a device share that context: a rank launching some
+// kernel for the first time would wait for a peer's k_comm_wait, which waits for that rank's signal — stuck until
+// the timeout.  Ranks on one device therefore need CUDA_MODULE_LOADING=EAGER (every kernel loaded up front).
+static bool lazy_module_loading() {
+  void* fn = nullptr;
+  cudaDriverEntryPointQueryResult q;
+  if (cudaGetDriverEntryPoint("cuModuleGetLoadingMode", &fn, cudaEnableDefault, &q) != cudaSuccess || !fn) {
+    cudaGetLastError();
+    return false;
+  }
+  CUmoduleLoadingMode mode;
+  return ((CUresult(*)(CUmoduleLoadingMode*))fn)(&mode) == CUDA_SUCCESS && mode == CU_MODULE_LAZY_LOADING;
+}
+
 int32_t comm_connect(Ctx* ctx, const unsigned char* blobs) {
   Comm* c = ctx->comm;
   if (!c) { set_error("comm_connect: dbsp_comm_create first"); return DBSP_ERR_INVALID; }
@@ -336,6 +352,11 @@ int32_t comm_connect(Ctx* ctx, const unsigned char* blobs) {
           return DBSP_ERR_CUDA;
         }
         cudaGetLastError();
+      } else if (lazy_module_loading()) {
+        set_error("comm_connect: ranks " + std::to_string(c->rank) + " and " + std::to_string(p) + " share device " +
+                  std::to_string(b.device) + ", which needs CUDA_MODULE_LOADING=EAGER in the environment (under lazy "
+                  "loading a rank's first launch of a kernel waits for a peer's kernel that waits for this rank)");
+        return DBSP_ERR_UNSUPPORTED;
       }
       c->peer[p] = (char*)(size_t)b.base;
     } else {

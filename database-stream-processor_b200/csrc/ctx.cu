@@ -45,8 +45,17 @@ ProfScope::~ProfScope() {
   if (idx >= 0) cudaEventRecord(c->prof[idx].b, c->stream);
 }
 
-static const size_t SLAB_BYTES = (size_t)8 << 30;   // 8 GiB per cudaMalloc
 static const size_t ALIGN = 512;
+// Bytes of one pool cudaMalloc: 8 GiB, or DBSP_POOL_SLAB_MB when set (several contexts sharing one device, e.g. one
+// per worker thread, would otherwise each start with 8 GiB).  A larger request still gets a slab of its own size.
+static size_t slab_bytes() {
+  static const size_t s = [] {
+    const char* e = getenv("DBSP_POOL_SLAB_MB");
+    const double mb = e ? atof(e) : 0.0;
+    return mb > 0 ? ((size_t)(mb * 1048576.0) + ALIGN - 1) & ~(ALIGN - 1) : (size_t)8 << 30;
+  }();
+  return s;
+}
 
 void pool_release_all(Ctx* ctx) {
   for (auto& kv : ctx->slabs) cudaFree(kv.first);
@@ -100,7 +109,7 @@ int32_t dev_alloc(Ctx* ctx, size_t bytes, BufP* out) {
   double t0 = now_us();
   auto it = ctx->free_by_size.lower_bound(need);
   if (it == ctx->free_by_size.end()) {
-    size_t slab = need > SLAB_BYTES ? need : SLAB_BYTES;
+    size_t slab = std::max(need, slab_bytes());
     void* p = nullptr;
     cudaError_t e = cudaMalloc(&p, slab);
     while (e != cudaSuccess && slab > need) {   // not enough room for a full slab: shrink towards the request

@@ -370,13 +370,18 @@ def canon(schema, cols, weights):
 def assert_batch_is(b, expect, what=""):
     """Backend batch `b` == the model's result: a Z, or (cols, weights) from consolidate_np."""
     if isinstance(expect, Z):
-        schema = expect.schema
+        assert b.schema == expect.schema, f"{what}: schema {b.schema} != {expect.schema}"
+    assert_download_is(b.schema, b.download(), expect, what)
+
+
+def assert_download_is(schema, got, expect, what=""):
+    """A batch of `schema` already downloaded (Batch.download()) == the model's result: a Z, or (cols, weights)
+    from consolidate_np."""
+    if isinstance(expect, Z):
         cols, w = flat(schema, expect)
     else:
-        schema = b.schema
         cols, w = expect
-    assert b.schema == schema, f"{what}: schema {b.schema} != {schema}"
-    want, got = canon(schema, cols, w), b.download()
+    want = canon(schema, cols, w)
     assert len(got["diffs"]) == len(want["diffs"]), f"{what}: {len(got['diffs'])} tuples, model has {len(want['diffs'])}"
     for part in ("keys", "vals"):
         for i, (x, y) in enumerate(zip(got[part], want[part])):

@@ -383,6 +383,8 @@ def assert_download_is(schema, got, expect, what=""):
         cols, w = expect
     want = canon(schema, cols, w)
     assert len(got["diffs"]) == len(want["diffs"]), f"{what}: {len(got['diffs'])} tuples, model has {len(want['diffs'])}"
+    for part in ("keys", "vals"):   # a download missing a lane must not pass by zip's truncation
+        assert len(got[part]) == len(want[part]), f"{what}: {len(got[part])} {part} lanes, model has {len(want[part])}"
     for part in ("keys", "vals"):
         for i, (x, y) in enumerate(zip(got[part], want[part])):
             assert np.array_equal(x, y), f"{what}: {part} lane {i} differs from the model"

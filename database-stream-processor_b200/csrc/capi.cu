@@ -5,6 +5,7 @@
 #include <cstdlib>
 
 #include "ops.cuh"
+#include "validate.h"
 
 const char* get_error();
 void print_host_stats(Ctx* c);
@@ -22,11 +23,38 @@ static inline dbsp_batch* H(Batch* b) { return (dbsp_batch*)b; }
 
 // every entry point makes the context's device current: a host may drive several contexts (GPUs) from one
 // process, one per worker thread (INTEGRATION.md §3)
-#define ENTER(c) CUDA_TRY(cudaSetDevice((c)->device))
 #define CHECK_ARG(c, msg)                 \
   do {                                    \
     if (!(c)) { set_error(msg); return DBSP_ERR_INVALID; } \
   } while (0)
+// The error contract of include/dbsp_b200.h: every argument is checked on the host before the call allocates, copies
+// or launches anything.  WHAT is the call's name without the prefix; the texts name the call and the argument.
+#define WHAT (__func__ + 5)
+#define NOT_NULL(p, name) CHECK_ARG((p) != nullptr, std::string(WHAT) + ": " name " is NULL")
+#define REFUSE(text)                                                  \
+  do {                                                                \
+    const std::string m__ = (text);                                   \
+    if (!m__.empty()) { set_error(m__); return DBSP_ERR_INVALID; }   \
+  } while (0)
+#define ENTER(c)        \
+  NOT_NULL(c, "ctx");   \
+  CUDA_TRY(cudaSetDevice((c)->device))
+namespace dv = dbsp_validate;
+// Row indices are 32-bit on the device: a batch of 2^32-1 or more rows is refused, never wrapped.
+#define ROWS32(n)                                                                                \
+  do {                                                                                           \
+    if ((u64)(n) >= 0xffffffffull) {                                                             \
+      set_error(std::string(WHAT) + ": n = " + std::to_string(n) + ": 2^32-1 or more rows in one batch; split the batch"); \
+      return DBSP_ERR_UNSUPPORTED;                                                               \
+    }                                                                                            \
+  } while (0)
+// host columns of a table or batch: the array and, when there are rows, each column the call reads
+static std::string valid_cols(const char* what, const u64* const* cols, int ncols, u64 n, unsigned mask = ~0u) {
+  if (!cols) return std::string(what) + ": cols is NULL";
+  for (int l = 0; n && l < ncols; l++)
+    if (((mask >> l) & 1) && !cols[l]) return std::string(what) + ": cols[" + std::to_string(l) + "] is NULL";
+  return "";
+}
 
 // Stage host columns on the device (stream-ordered).  Host memory may be
 // pageable; pinned memory makes the copy asynchronous.
@@ -340,6 +368,8 @@ extern "C" {
 const char* dbsp_last_error(void) { return get_error(); }
 
 int32_t dbsp_ctx_create(int32_t device, dbsp_ctx** out) {
+  NOT_NULL(out, "out");
+  CHECK_ARG(device >= 0, "ctx_create: device is negative");
   int count = 0;
   cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess || count == 0 || device >= count) {
@@ -418,14 +448,16 @@ int32_t dbsp_ctx_stats(dbsp_ctx* c, uint64_t* k, uint64_t* h2d, uint64_t* d2h, i
   return DBSP_OK;
 }
 int32_t dbsp_ctx_sync_stats(dbsp_ctx* c, uint64_t* n_waits, double* wait_us, int32_t reset) {
+  NOT_NULL(c, "ctx");
   if (n_waits) *n_waits = c->n_sync;
   if (wait_us) *wait_us = c->t_sync_us;
   if (reset) { c->n_sync = 0; c->t_sync_us = 0; }
   return DBSP_OK;
 }
-void* dbsp_ctx_stream(dbsp_ctx* c) { return (void*)c->stream; }
+void* dbsp_ctx_stream(dbsp_ctx* c) { return c ? (void*)c->stream : nullptr; }
 
 int32_t dbsp_ctx_profile(dbsp_ctx* c, int32_t enable) { ENTER(c);
+  CHECK_ARG(enable >= 0 && enable <= 2, "ctx_profile: enable must be 0, 1 or 2");
   if (enable == 2) { c->prof_on = false; return DBSP_OK; }   // pause: keep what was collected, record nothing more
   CUDA_TRY(cudaStreamSynchronize(c->stream));
   for (auto& r : c->prof) { c->ev_pool.push_back(r.a); c->ev_pool.push_back(r.b); }
@@ -454,8 +486,11 @@ int32_t dbsp_ctx_profile_read(dbsp_ctx* c, int32_t id, char* name32, uint64_t* l
 
 int32_t dbsp_batch_from_tuples(dbsp_ctx* ctx, const dbsp_schema* s, const uint64_t* const* cols, const int64_t* w,
                                uint64_t n, int32_t on_device, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_schema(s, WHAT));
   int L = s->n_key_lanes + s->n_val_lanes;
-  CHECK_ARG(L >= 1 && L <= MAXL, "schema must have 1..8 lanes");
+  REFUSE(valid_cols(WHAT, cols, L, n));
+  ROWS32(n);
   BufP hold;
   Cols dc;
   const i64* dw;
@@ -468,7 +503,11 @@ int32_t dbsp_batch_from_tuples(dbsp_ctx* ctx, const dbsp_schema* s, const uint64
 
 int32_t dbsp_batch_from_table(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n_cols, const int64_t* w, uint64_t n,
                               int32_t on_device, const dbsp_proj* proj, dbsp_batch** out) { ENTER(ctx);
-  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "table must have 1..8 columns");
+  NOT_NULL(out, "out");
+  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "batch_from_table: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
+  REFUSE(dv::valid_proj(proj, (int)n_cols, (int)n_cols, (int)n_cols, WHAT));
+  REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, dv::proj_table_mask(*proj)));
+  ROWS32(n);
   BufP hold;
   Cols dc;
   const i64* dw;
@@ -486,20 +525,32 @@ struct dbsp_upload {
   const i64* dw;
   u64 n;
   int n_cols;
+  unsigned col_mask;
   cudaEvent_t done;
 };
 
-uint32_t dbsp_proj_table_mask(const dbsp_proj* proj) { return proj_used_mask(*proj, 0); }
+uint32_t dbsp_proj_table_mask(const dbsp_proj* proj) {
+  if (!dv::valid_proj(proj, MAXL, MAXL, MAXL, "proj_table_mask").empty()) return 0;
+  return dv::proj_table_mask(*proj);
+}
 
 int32_t dbsp_upload_begin(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n_cols, uint32_t col_mask,
                           const int64_t* w, uint64_t n, dbsp_upload** out) { ENTER(ctx);
-  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "table must have 1..8 columns");
+  NOT_NULL(out, "out");
+  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "upload_begin: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
+  REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, col_mask));
+  ROWS32(n);
   dbsp_upload* u = new dbsp_upload();
   u->ctx = ctx;
   u->n = n;
   u->n_cols = (int)n_cols;
+  u->col_mask = col_mask;
   u->dw = nullptr;
   for (int l = 0; l < MAXL; l++) u->dc.c[l] = nullptr;
+  u->done = nullptr;
+  // a failure below must not leak the handle, its buffer or its event; copies already queued read the caller's
+  // columns, so they are drained before the error returns
+  auto queue = [&]() -> int32_t {
   CUDA_TRY(cudaEventCreateWithFlags(&u->done, cudaEventDisableTiming));
   if (n) {
     u64 cap = (n + 32) & ~31ull;
@@ -525,11 +576,28 @@ int32_t dbsp_upload_begin(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n
     }
   }
   CUDA_TRY(cudaEventRecord(u->done, ctx->copy_stream));
+  return DBSP_OK;
+  };
+  const int32_t rc = queue();
+  if (rc != DBSP_OK) {
+    cudaStreamSynchronize(ctx->copy_stream);
+    if (u->done) cudaEventDestroy(u->done);
+    delete u;
+    return rc;
+  }
   *out = u;
   return DBSP_OK;
 }
 
 int32_t dbsp_batch_from_upload(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_proj* proj, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(u, "upload");
+  CHECK_ARG(u->ctx == ctx, "batch_from_upload: upload belongs to another context");
+  REFUSE(dv::valid_proj(proj, u->n_cols, u->n_cols, u->n_cols, WHAT));
+  {
+    const unsigned missing = dv::proj_table_mask(*proj) & ~u->col_mask;
+    CHECK_ARG(missing == 0, "batch_from_upload: proj reads column " + std::to_string(__builtin_ctz(missing | 0x100u)) + ", which col_mask left out of the upload");
+  }
   CUDA_TRY(cudaStreamWaitEvent(ctx->stream, u->done, 0));   // compute stream waits for the copy
   Batch* b = nullptr;
   TRY(project_and_consolidate(ctx, u->dc, 0, u->n_cols, u->dw, u->n, *proj, &b));
@@ -549,7 +617,12 @@ int32_t dbsp_upload_free(dbsp_upload* u) {
 
 int32_t dbsp_batch_from_sorted(dbsp_ctx* ctx, const dbsp_schema* s, const uint64_t* const* cols, const int64_t* w,
                                uint64_t n, int32_t on_device, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_schema(s, WHAT));
   int L = s->n_key_lanes + s->n_val_lanes;
+  REFUSE(valid_cols(WHAT, cols, L, n));
+  CHECK_ARG(n == 0 || w != nullptr, "batch_from_sorted: weights is NULL (consolidated rows carry their weights)");
+  ROWS32(n);
   if (n == 0) { *out = H(batch_new_empty(ctx, *s)); return DBSP_OK; }
   Batch* b;
   MCols oc;
@@ -586,9 +659,10 @@ static int32_t batcher_enqueue(Ctx* ctx, Batcher* q, Batch* b) {
   }
   return DBSP_OK;
 }
-int32_t dbsp_batcher_new(dbsp_ctx*, const dbsp_schema* s, dbsp_batcher** out) {
-  int L = s->n_key_lanes + s->n_val_lanes;
-  CHECK_ARG(L >= 1 && L <= MAXL, "schema must have 1..8 lanes");
+int32_t dbsp_batcher_new(dbsp_ctx* ctx, const dbsp_schema* s, dbsp_batcher** out) {
+  NOT_NULL(ctx, "ctx");
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_schema(s, WHAT));
   Batcher* q = new Batcher();
   q->s = *s;
   *out = (dbsp_batcher*)q;
@@ -596,7 +670,10 @@ int32_t dbsp_batcher_new(dbsp_ctx*, const dbsp_schema* s, dbsp_batcher** out) {
 }
 int32_t dbsp_batcher_push(dbsp_ctx* ctx, dbsp_batcher* bq, const uint64_t* const* cols, const int64_t* w, uint64_t n,
                           int32_t on_device) { ENTER(ctx);
+  NOT_NULL(bq, "batcher");
   Batcher* q = (Batcher*)bq;
+  REFUSE(valid_cols(WHAT, cols, q->s.n_key_lanes + q->s.n_val_lanes, n));
+  ROWS32(n);
   if (n == 0) return DBSP_OK;
   dbsp_batch* b = nullptr;
   TRY(dbsp_batch_from_tuples(ctx, &q->s, cols, w, n, on_device, &b));
@@ -604,14 +681,19 @@ int32_t dbsp_batcher_push(dbsp_ctx* ctx, dbsp_batcher* bq, const uint64_t* const
 }
 int32_t dbsp_batcher_push_consolidated(dbsp_ctx* ctx, dbsp_batcher* bq, const uint64_t* const* cols, const int64_t* w,
                                        uint64_t n, int32_t on_device) { ENTER(ctx);
+  NOT_NULL(bq, "batcher");
   Batcher* q = (Batcher*)bq;
+  REFUSE(valid_cols(WHAT, cols, q->s.n_key_lanes + q->s.n_val_lanes, n));
+  ROWS32(n);
   if (n == 0) return DBSP_OK;
-  CHECK_ARG(w != nullptr, "push_consolidated: weights required");
+  CHECK_ARG(w != nullptr, "batcher_push_consolidated: weights is NULL (consolidated rows carry their weights)");
   dbsp_batch* b = nullptr;
   TRY(dbsp_batch_from_sorted(ctx, &q->s, cols, w, n, on_device, &b));
   return batcher_enqueue(ctx, q, B(b));
 }
 int32_t dbsp_batcher_tuples(const dbsp_batcher* bq, uint64_t* n) {
+  NOT_NULL(bq, "batcher");
+  NOT_NULL(n, "n_tuples");
   u64 t = 0;
   for (Batch* b : ((const Batcher*)bq)->queue) t += b->n;
   *n = t;
@@ -625,6 +707,8 @@ int32_t dbsp_batcher_free(dbsp_batcher* bq) {
   return DBSP_OK;
 }
 int32_t dbsp_batcher_seal(dbsp_ctx* ctx, dbsp_batcher* bq, dbsp_batch** out) { ENTER(ctx);   // finish_into (:251-265) + Builder
+  NOT_NULL(bq, "batcher");
+  NOT_NULL(out, "out");
   Batcher* q = (Batcher*)bq;
   while (q->queue.size() >= 2) {
     Batch* y = q->queue.back(); q->queue.pop_back();
@@ -644,11 +728,17 @@ int32_t dbsp_batcher_seal(dbsp_ctx* ctx, dbsp_batcher* bq, dbsp_batch** out) { E
 }
 
 int32_t dbsp_batch_empty(dbsp_ctx* ctx, const dbsp_schema* s, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_schema(s, WHAT));
   *out = H(batch_new_empty(ctx, *s));
   return DBSP_OK;
 }
 
 int32_t dbsp_batch_merge(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(a, "a");
+  NOT_NULL(b, "b");
+  CHECK_ARG(dv::same_schema(B(a)->s, B(b)->s), std::string(WHAT) + ": a and b differ in schema");
   Batch* o = nullptr;
   TRY(merge_batches(ctx, B(a), B(b), &o));
   *out = H(o);
@@ -657,6 +747,10 @@ int32_t dbsp_batch_merge(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b
 
 int32_t dbsp_batch_merge_bounded(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b, const uint64_t* vb,
                                  dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(a, "a");
+  NOT_NULL(b, "b");
+  CHECK_ARG(dv::same_schema(B(a)->s, B(b)->s), std::string(WHAT) + ": a and b differ in schema");
   Batch* o = nullptr;
   TRY(merge_bounded(ctx, B(a), B(b), vb, &o));
   *out = H(o);
@@ -664,6 +758,9 @@ int32_t dbsp_batch_merge_bounded(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_
 }
 
 int32_t dbsp_batch_truncate_keys_below(dbsp_ctx* ctx, const dbsp_batch* b, const uint64_t* key, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  CHECK_ARG(key != nullptr || B(b)->s.n_key_lanes == 0, "batch_truncate_keys_below: key is NULL");
   u64 pos;
   TRY(batch_lower_bound(ctx, B(b), key, &pos));
   if (pos == 0) { batch_ref(B(b)); *out = (dbsp_batch*)b; return DBSP_OK; }
@@ -672,7 +769,10 @@ int32_t dbsp_batch_truncate_keys_below(dbsp_ctx* ctx, const dbsp_batch* b, const
 }
 
 int32_t dbsp_merger_new(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b, const uint64_t* vb, dbsp_merger** out) { ENTER(ctx);
-  CHECK_ARG(memcmp(&B(a)->s, &B(b)->s, sizeof(dbsp_schema)) == 0, "merger_new: schema mismatch");
+  NOT_NULL(out, "out");
+  NOT_NULL(a, "a");
+  NOT_NULL(b, "b");
+  CHECK_ARG(dv::same_schema(B(a)->s, B(b)->s), std::string(WHAT) + ": a and b differ in schema");
   Merger* m = new Merger();
   m->ctx = ctx;
   m->a = B(a);
@@ -688,6 +788,8 @@ int32_t dbsp_merger_new(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b,
 }
 
 int32_t dbsp_merger_work(dbsp_ctx* ctx, dbsp_merger* mm, int64_t* fuel) { ENTER(ctx);
+  NOT_NULL(mm, "merger");
+  NOT_NULL(fuel, "fuel");
   Merger* m = (Merger*)mm;
   if (!m->complete() && *fuel > 0) {
     u64 na, nb;
@@ -720,8 +822,10 @@ int32_t dbsp_merger_free(dbsp_merger* mm) {
 }
 
 int32_t dbsp_merger_done(dbsp_ctx* ctx, dbsp_merger* mm, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(mm, "merger");
+  NOT_NULL(out, "out");
   Merger* m = (Merger*)mm;
-  CHECK_ARG(m->complete(), "merger_done: merge not complete");
+  CHECK_ARG(m->complete(), "merger_done: merger: the merge is not complete (merger_work left fuel <= 0)");
   Batch* o = nullptr;
   TRY(batch_concat(ctx, m->a->s, m->chunks, &o));   // on failure the merger stays owned by the caller
   dbsp_merger_free(mm);
@@ -730,6 +834,8 @@ int32_t dbsp_merger_done(dbsp_ctx* ctx, dbsp_merger* mm, dbsp_batch** out) { ENT
 }
 
 int32_t dbsp_batch_neg(dbsp_ctx* ctx, const dbsp_batch* a, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(a, "batch");
   Batch* o = nullptr;
   TRY(op_neg(ctx, B(a), &o));
   *out = H(o);
@@ -737,8 +843,10 @@ int32_t dbsp_batch_neg(dbsp_ctx* ctx, const dbsp_batch* a, dbsp_batch** out) { E
 }
 
 int32_t dbsp_batch_reindex(dbsp_ctx* ctx, const dbsp_batch* a, uint32_t nk, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(a, "batch");
   const Batch* x = B(a);
-  CHECK_ARG((int)nk <= x->nl(), "reindex: too many key lanes");
+  CHECK_ARG(nk <= (uint32_t)x->nl(), "batch_reindex: n_key_lanes = " + std::to_string(nk) + ": the batch has " + std::to_string(x->nl()) + " lanes");
   Batch* v = new Batch();
   v->s = x->s;
   v->s.n_key_lanes = (uint8_t)nk;
@@ -753,18 +861,31 @@ int32_t dbsp_batch_reindex(dbsp_ctx* ctx, const dbsp_batch* a, uint32_t nk, dbsp
   return DBSP_OK;
 }
 
-int32_t dbsp_batch_len(const dbsp_batch* b, uint64_t* n) { *n = B(b)->n; return DBSP_OK; }
+int32_t dbsp_batch_len(const dbsp_batch* b, uint64_t* n) {
+  NOT_NULL(b, "batch");
+  NOT_NULL(n, "n_tuples");
+  *n = B(b)->n;
+  return DBSP_OK;
+}
 int32_t dbsp_batch_key_count(dbsp_ctx* ctx, const dbsp_batch* b, uint64_t* n) { ENTER(ctx);
+  NOT_NULL(b, "batch");
+  NOT_NULL(n, "n_keys");
   Batch* x = B(b);
   if (x->s.n_val_lanes == 0) { *n = x->n; return DBSP_OK; }
   TRY(batch_build_csr(ctx, x));
   *n = x->nkeys;
   return DBSP_OK;
 }
-int32_t dbsp_batch_schema(const dbsp_batch* b, dbsp_schema* out) { *out = B(b)->s; return DBSP_OK; }
+int32_t dbsp_batch_schema(const dbsp_batch* b, dbsp_schema* out) {
+  NOT_NULL(b, "batch");
+  NOT_NULL(out, "out");
+  *out = B(b)->s;
+  return DBSP_OK;
+}
 
 int32_t dbsp_batch_download_csr(dbsp_ctx* ctx, const dbsp_batch* bb, uint64_t* const* keys, uint64_t* offs,
                                 uint64_t* const* vals, int64_t* diffs) { ENTER(ctx);
+  NOT_NULL(bb, "batch");
   Batch* b = B(bb);
   cudaStream_t st = ctx->stream;
   int nk = b->s.n_key_lanes, nv = b->s.n_val_lanes;
@@ -802,6 +923,8 @@ struct dbsp_download {
 };
 int32_t dbsp_batch_download_begin(dbsp_ctx* ctx, const dbsp_batch* bb, uint64_t* const* cols, int64_t* diffs,
                                   dbsp_download** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(bb, "batch");
   Batch* b = B(bb);
   cudaEvent_t done;
   CUDA_TRY(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
@@ -853,6 +976,8 @@ int32_t dbsp_download_finish(dbsp_download* d) {
 }
 
 int32_t dbsp_batch_device_columns(const dbsp_batch* b, const uint64_t** cols, const int64_t** w) {
+  NOT_NULL(b, "batch");
+  NOT_NULL(cols, "cols");
   const Batch* x = B(b);
   for (int l = 0; l < x->nl(); l++) cols[l] = x->col[l];
   if (w) *w = x->w;
@@ -860,6 +985,9 @@ int32_t dbsp_batch_device_columns(const dbsp_batch* b, const uint64_t** cols, co
 }
 
 int32_t dbsp_batch_last_key(dbsp_ctx* ctx, const dbsp_batch* b, uint64_t* key, int32_t* valid) { ENTER(ctx);
+  NOT_NULL(b, "batch");
+  NOT_NULL(valid, "valid");
+  CHECK_ARG(key != nullptr || B(b)->s.n_key_lanes == 0, "batch_last_key: key is NULL");
   const Batch* x = B(b);
   *valid = x->n > 0;
   if (!x->n) return DBSP_OK;
@@ -872,10 +1000,21 @@ int32_t dbsp_batch_last_key(dbsp_ctx* ctx, const dbsp_batch* b, uint64_t* key, i
   return DBSP_OK;
 }
 
-int32_t dbsp_batch_clone(const dbsp_batch* b, dbsp_batch** out) { batch_ref(B(b)); *out = (dbsp_batch*)b; return DBSP_OK; }
-int32_t dbsp_batch_free(dbsp_batch* b) { batch_unref(B(b)); return DBSP_OK; }
+int32_t dbsp_batch_clone(const dbsp_batch* b, dbsp_batch** out) {
+  NOT_NULL(b, "batch");
+  NOT_NULL(out, "out");
+  batch_ref(B(b));
+  *out = (dbsp_batch*)b;
+  return DBSP_OK;
+}
+int32_t dbsp_batch_free(dbsp_batch* b) {
+  if (b) batch_unref(B(b));
+  return DBSP_OK;
+}
 
 int32_t dbsp_spine_new(dbsp_ctx* ctx, const dbsp_schema* s, dbsp_spine** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_schema(s, WHAT));
   dbsp_spine* sp = new dbsp_spine();
   sp->s = *s;
   sp->ctx = ctx;
@@ -883,10 +1022,14 @@ int32_t dbsp_spine_new(dbsp_ctx* ctx, const dbsp_schema* s, dbsp_spine** out) { 
   return DBSP_OK;
 }
 int32_t dbsp_spine_insert(dbsp_ctx* ctx, dbsp_spine* s, const dbsp_batch* b) { ENTER(ctx);
-  CHECK_ARG(memcmp(&s->s, &B(b)->s, sizeof(dbsp_schema)) == 0, "spine_insert: schema mismatch");
+  NOT_NULL(s, "spine");
+  NOT_NULL(b, "batch");
+  CHECK_ARG(dv::same_schema(s->s, B(b)->s), "spine_insert: spine and batch differ in schema");
   return spine_insert(ctx, s, B(b));
 }
 int32_t dbsp_spine_consolidate(dbsp_ctx* ctx, dbsp_spine* s, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(s, "spine");
+  NOT_NULL(out, "out");
   // A consolidated read of the trace: the merge of everything a cursor sees, with the value bound applied.
   // Trace::consolidate (:583-600) consumes the trace; this leaves the layers (and their merge schedule) as they are.
   const u64* vb = s->has_vbound ? s->vbound : nullptr;
@@ -902,6 +1045,8 @@ int32_t dbsp_spine_consolidate(dbsp_ctx* ctx, dbsp_spine* s, dbsp_batch** out) {
   return DBSP_OK;
 }
 int32_t dbsp_spine_truncate_keys_below(dbsp_ctx* ctx, dbsp_spine* s, const uint64_t* key) { ENTER(ctx);
+  NOT_NULL(s, "spine");
+  CHECK_ARG(key != nullptr || s->s.n_key_lanes == 0, "spine_truncate_keys_below: key is NULL");
   bool raise = !s->has_bound;
   if (!raise) {   // the bound only grows (spine_fueled.rs:223-233)
     for (int l = 0; l < s->s.n_key_lanes; l++) {
@@ -925,7 +1070,10 @@ int32_t dbsp_spine_truncate_keys_below(dbsp_ctx* ctx, dbsp_spine* s, const uint6
   spine_refresh_view(s);
   return DBSP_OK;
 }
-int32_t dbsp_spine_truncate_values_below(dbsp_ctx*, dbsp_spine* s, const uint64_t* val) {
+int32_t dbsp_spine_truncate_values_below(dbsp_ctx* ctx, dbsp_spine* s, const uint64_t* val) {
+  NOT_NULL(ctx, "ctx");
+  NOT_NULL(s, "spine");
+  CHECK_ARG(val != nullptr || s->s.n_val_lanes == 0, "spine_truncate_values_below: val is NULL");
   int nk = s->s.n_key_lanes, nv = s->s.n_val_lanes;
   bool raise = !s->has_vbound;
   if (!raise) {   // the bound only grows (spine_fueled.rs:644-652)
@@ -940,10 +1088,13 @@ int32_t dbsp_spine_truncate_values_below(dbsp_ctx*, dbsp_spine* s, const uint64_
   return DBSP_OK;
 }
 int32_t dbsp_spine_exert(dbsp_ctx* ctx, dbsp_spine* s, int64_t* effort) { ENTER(ctx);
+  NOT_NULL(s, "spine");
+  NOT_NULL(effort, "effort");
   i64 e = *effort;
   return spine_exert(ctx, s, &e);
 }
 int32_t dbsp_spine_len(const dbsp_spine* s, uint64_t* n, uint32_t* nb) {
+  NOT_NULL(s, "spine");
   u64 t = 0;
   for (Batch* b : s->batches) t += b->n;
   if (n) *n = t;
@@ -980,17 +1131,20 @@ static int32_t save_batch(Ctx* ctx, FILE* f, const Batch* b, std::vector<u64>& s
   }
   return DBSP_OK;
 }
-static int32_t load_batch(Ctx* ctx, FILE* f, const dbsp_schema& sc, Batch** out, std::vector<u64>& stage) {
+// batch `which` (0 = a, 1 = b) of a layer of kind `kind`; `file_bytes` is the size of the whole file
+static int32_t load_batch(Ctx* ctx, FILE* f, u64 file_bytes, const dbsp_schema& sc, u64 kind, int which, Batch** out,
+                          std::vector<u64>& stage) {
   u64 present = 0, n = 0;
   *out = nullptr;
-  if (!fread_all(f, &present, 8) || !fread_all(f, &n, 8)) { set_error("spine_load: truncated file"); return DBSP_ERR_INVALID; }
+  if (!fread_all(f, &present, 8) || !fread_all(f, &n, 8)) { set_error("spine_load: truncated file (batch header)"); return DBSP_ERR_INVALID; }
+  const int L = sc.n_key_lanes + sc.n_val_lanes;
+  REFUSE(dv::valid_snapshot_batch(kind, which, present, n, L, file_bytes - (u64)ftell(f)));
   if (!present) return DBSP_OK;
   if (!n) { *out = batch_new_empty(ctx, sc); return DBSP_OK; }
   Batch* b;
   MCols oc;
   i64* ow;
   TRY(batch_alloc(ctx, sc, n, &b, &oc, &ow));
-  const int L = sc.n_key_lanes + sc.n_val_lanes;
   for (int l = 0; l <= L; l++) {
     u64* dst = l < L ? oc.c[l] : (u64*)ow;
     for (u64 off = 0; off < n; off += stage.size()) {
@@ -1002,11 +1156,23 @@ static int32_t load_batch(Ctx* ctx, FILE* f, const dbsp_schema& sc, Batch** out,
       ctx->h2d_bytes += m * 8;
     }
   }
+  // the rows become a batch of the trace as they are: they must be what a batch is — ordered, free of duplicate
+  // rows and of zero weights — or every later merge and probe of the trace would be silently wrong
+  u64 inv = 0, dup = 0, zero = 0;
+  int32_t rc = rows_census(ctx, sc, b->cols(), b->w, n, &inv, &dup, &zero);
+  if (rc == DBSP_OK && (inv || dup || zero)) {
+    set_error("spine_load: rows of a batch are not consolidated (" + std::to_string(inv) + " out of order, " + std::to_string(dup) +
+              " duplicates, " + std::to_string(zero) + " zero weights)");
+    rc = DBSP_ERR_INVALID;
+  }
+  if (rc != DBSP_OK) { batch_unref(b); return rc; }
   *out = b;
   return DBSP_OK;
 }
 
 int32_t dbsp_spine_save(dbsp_ctx* ctx, const dbsp_spine* s, const char* path) { ENTER(ctx);
+  NOT_NULL(s, "spine");
+  NOT_NULL(path, "path");
   FILE* f = fopen(path, "wb");
   if (!f) { set_error(std::string("spine_save: cannot open ") + path); return DBSP_ERR_INVALID; }
   std::vector<u64> stage((size_t)8 << 20);   // 64 MiB staging
@@ -1026,36 +1192,46 @@ int32_t dbsp_spine_save(dbsp_ctx* ctx, const dbsp_spine* s, const char* path) { 
   return rc;
 }
 int32_t dbsp_spine_load(dbsp_ctx* ctx, const char* path, dbsp_spine** out) { ENTER(ctx);
+  NOT_NULL(path, "path");
+  NOT_NULL(out, "out");
   FILE* f = fopen(path, "rb");
   if (!f) { set_error(std::string("spine_load: cannot open ") + path); return DBSP_ERR_INVALID; }
-  std::vector<u64> stage((size_t)8 << 20);
-  char magic[8];
-  u64 hdr[4];
   dbsp_spine* sp = new dbsp_spine();
   sp->ctx = ctx;
-  int32_t rc = DBSP_OK;
-  if (!fread_all(f, magic, 8) || memcmp(magic, SPINE_MAGIC, 8) != 0 || !fread_all(f, &sp->s, sizeof(dbsp_schema)) ||
-      !fread_all(f, hdr, sizeof(hdr)) || !fread_all(f, sp->bound, sizeof(u64) * MAXL) || !fread_all(f, sp->vbound, sizeof(u64) * MAXL)) {
-    set_error("spine_load: not a spine snapshot");
-    rc = DBSP_ERR_INVALID;
-  }
-  if (rc == DBSP_OK) {
+  // everything is checked as it is read and before anything is allocated for it (validate.h); a refused file
+  // leaves nothing behind
+  auto load = [&]() -> int32_t {
+    u64 file_bytes = 0;
+    if (fseek(f, 0, SEEK_END) == 0) { file_bytes = (u64)ftell(f); rewind(f); }
+    char magic[8];
+    u64 hdr[4];
+    if (!fread_all(f, magic, 8) || memcmp(magic, SPINE_MAGIC, 8) != 0) { set_error("spine_load: not a spine snapshot (magic)"); return DBSP_ERR_INVALID; }
+    if (!fread_all(f, &sp->s, sizeof(dbsp_schema)) || !fread_all(f, hdr, sizeof(hdr)) || !fread_all(f, sp->bound, sizeof(u64) * MAXL) ||
+        !fread_all(f, sp->vbound, sizeof(u64) * MAXL)) {
+      set_error("spine_load: truncated file (header)");
+      return DBSP_ERR_INVALID;
+    }
+    REFUSE(dv::valid_snapshot_header(sp->s, hdr));
     sp->has_bound = hdr[0] != 0;
     sp->has_vbound = hdr[1] != 0;
     sp->effort = hdr[2] ? hdr[2] : 1;
-    if (hdr[3] > 64) { set_error("spine_load: corrupt layer count"); rc = DBSP_ERR_INVALID; }
-  }
-  for (u64 i = 0; rc == DBSP_OK && i < hdr[3]; i++) {
-    u64 lh[2];
-    if (!fread_all(f, lh, sizeof(lh)) || lh[0] > (u64)SpineLevel::COMPLETE) { set_error("spine_load: truncated file"); rc = DBSP_ERR_INVALID; break; }
-    SpineLevel l;
-    l.kind = (SpineLevel::Kind)lh[0];
-    l.remaining = (i64)lh[1];
-    rc = load_batch(ctx, f, sp->s, &l.a, stage);
-    if (rc == DBSP_OK) rc = load_batch(ctx, f, sp->s, &l.b, stage);
-    if (rc == DBSP_OK && l.kind == SpineLevel::IN_PROGRESS && (!l.a || !l.b)) { set_error("spine_load: corrupt layer"); rc = DBSP_ERR_INVALID; }
-    sp->merging.push_back(l);
-  }
+    std::vector<u64> stage((size_t)std::min<u64>((u64)8 << 20, file_bytes / 8 + 1));   // at most 64 MiB of staging
+    for (u64 i = 0; i < hdr[3]; i++) {
+      u64 lh[2];
+      if (!fread_all(f, lh, sizeof(lh))) { set_error("spine_load: truncated file (layer header)"); return DBSP_ERR_INVALID; }
+      REFUSE(dv::valid_snapshot_kind(lh[0]));
+      sp->merging.push_back(SpineLevel());   // owned by the spine from here on: released with it
+      SpineLevel& l = sp->merging.back();
+      TRY(load_batch(ctx, f, file_bytes, sp->s, lh[0], 0, &l.a, stage));
+      TRY(load_batch(ctx, f, file_bytes, sp->s, lh[0], 1, &l.b, stage));
+      REFUSE(dv::valid_snapshot_remaining(lh[1], l.a ? l.a->n : 0, l.b ? l.b->n : 0));
+      l.kind = (SpineLevel::Kind)lh[0];
+      l.remaining = (i64)lh[1];
+    }
+    if ((u64)ftell(f) != file_bytes) { set_error("spine_load: " + std::to_string(file_bytes - (u64)ftell(f)) + " trailing bytes after the last layer"); return DBSP_ERR_INVALID; }
+    return DBSP_OK;
+  };
+  const int32_t rc = load();
   fclose(f);
   if (rc != DBSP_OK) { spine_release(sp); delete sp; return rc; }
   spine_refresh_view(sp);
@@ -1069,33 +1245,91 @@ int32_t dbsp_spine_load(dbsp_ctx* ctx, const char* path, dbsp_spine** out) { ENT
   *out = H(o__);              \
   return DBSP_OK;
 
+// the two sides of a join: equal key lanes; proj reads the key, the left values and the right values
+static std::string valid_join(const char* what, const dbsp_schema& left, const dbsp_schema& right, const dbsp_proj* p) {
+  if (!dv::same_key_lanes(left, right)) return std::string(what) + ": the two inputs differ in key lanes (count or type)";
+  return dv::valid_proj(p, left.n_key_lanes, left.n_val_lanes, right.n_val_lanes, what);
+}
+
 int32_t dbsp_join_delta_trace(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* t, const dbsp_proj* p, int32_t dl,
-                              dbsp_batch** out) { ENTER(ctx); OUT1(op_join_delta_trace(ctx, B(d), t, p, dl, &o__)) }
+                              dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(d, "delta");
+  NOT_NULL(t, "trace");
+  REFUSE(dl ? valid_join(WHAT, B(d)->s, t->s, p) : valid_join(WHAT, t->s, B(d)->s, p));
+  OUT1(op_join_delta_trace(ctx, B(d), t, p, dl, &o__)) }
 int32_t dbsp_join_batches(dbsp_ctx* ctx, const dbsp_batch* l, const dbsp_batch* r, const dbsp_proj* p, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(l, "left");
+  NOT_NULL(r, "right");
+  REFUSE(valid_join(WHAT, B(l)->s, B(r)->s, p));
   OUT1(op_join_batches(ctx, B(l), B(r), p, &o__)) }
 int32_t dbsp_semijoin(dbsp_ctx* ctx, const dbsp_batch* pairs, const dbsp_batch* keys, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(pairs, "pairs");
+  NOT_NULL(keys, "keys");
+  CHECK_ARG(dv::same_key_lanes(B(pairs)->s, B(keys)->s), "semijoin: pairs and keys differ in key lanes (count or type)");
+  CHECK_ARG(B(keys)->s.n_val_lanes == 0, "semijoin: keys must be a batch without value lanes");
   OUT1(op_semijoin(ctx, B(pairs), B(keys), &o__)) }
 int32_t dbsp_aggregate_delta(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* in_tr, const dbsp_spine* out_tr,
-                             int32_t kind, dbsp_batch** out) { ENTER(ctx); OUT1(op_aggregate_delta(ctx, B(d), in_tr, out_tr, kind, &o__)) }
+                             int32_t kind, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(d, "delta");
+  NOT_NULL(in_tr, "in_trace");
+  NOT_NULL(out_tr, "out_trace");
+  REFUSE(dv::valid_aggregate(B(d)->s, in_tr->s, out_tr->s, kind));
+  OUT1(op_aggregate_delta(ctx, B(d), in_tr, out_tr, kind, &o__)) }
 int32_t dbsp_weigh(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_expr* f, int32_t mode, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || mode == DBSP_WEIGH_AVG, "weigh: mode = " + std::to_string(mode) + " is not a weigh mode");
+  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || B(b)->s.n_key_lanes < MAXL, "weigh: WEIGH_AVG adds a key lane and the batch already has 8");
+  CHECK_ARG(mode == DBSP_WEIGH_AVG || B(b)->s.n_key_lanes >= 1, "weigh: WEIGH_LINEAR of a batch without key lanes has no output lanes");
+  REFUSE(dv::valid_expr(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, "weigh: f"));
   OUT1(op_weigh(ctx, B(b), f, mode, &o__)) }
 int32_t dbsp_distinct_delta(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* i, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(d, "delta");
+  NOT_NULL(i, "delayed_integral");
+  CHECK_ARG(dv::same_schema(B(d)->s, i->s), "distinct_delta: delta and delayed_integral differ in schema");
   OUT1(op_distinct_delta(ctx, B(d), i, &o__)) }
-int32_t dbsp_stream_distinct(dbsp_ctx* ctx, const dbsp_batch* b, dbsp_batch** out) { ENTER(ctx); OUT1(op_stream_distinct(ctx, B(b), &o__)) }
+int32_t dbsp_stream_distinct(dbsp_ctx* ctx, const dbsp_batch* b, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  OUT1(op_stream_distinct(ctx, B(b), &o__)) }
 int32_t dbsp_window_delta(dbsp_ctx* ctx, const dbsp_spine* t, const dbsp_batch* d, int32_t has_prev, const uint64_t* s0,
                           const uint64_t* e0, const uint64_t* s1, const uint64_t* e1, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(t, "trace");
+  NOT_NULL(d, "delta");
+  CHECK_ARG(dv::same_schema(t->s, B(d)->s), "window_delta: trace and delta differ in schema");
+  CHECK_ARG(s1 && e1, "window_delta: start1 / end1 is NULL");
+  CHECK_ARG(!has_prev || (s0 && e0), "window_delta: start0 / end0 is NULL although has_prev is set");
+  if (!has_prev) { s0 = s1; e0 = e1; }   // never read by the operator's logic; keeps the copies below defined
   OUT1(op_window_delta(ctx, t, B(d), has_prev, s0, e0, s1, e1, &o__)) }
 int32_t dbsp_map_index(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_proj* p, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  REFUSE(dv::valid_proj(p, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT));
   OUT1(op_map_index(ctx, B(b), p, &o__)) }
 int32_t dbsp_shard_partition(dbsp_ctx* ctx, const dbsp_batch* b, uint32_t P, dbsp_batch** outs) { ENTER(ctx);
+  NOT_NULL(b, "batch");
+  NOT_NULL(outs, "outs");
+  CHECK_ARG(P >= 1 && P <= 64, "shard_partition: n_shards = " + std::to_string(P) + ": 1..64 shards");
   std::vector<Batch*> o(P, nullptr);
-  TRY(op_shard_partition(ctx, B(b), P, o.data()));
+  const int32_t rc = op_shard_partition(ctx, B(b), P, o.data());
+  if (rc != DBSP_OK) {
+    for (Batch* x : o) if (x) batch_unref(x);
+    return rc;
+  }
   for (uint32_t p = 0; p < P; p++) outs[p] = H(o[p]);
   return DBSP_OK;
 }
 
 int32_t dbsp_comm_create(dbsp_ctx* ctx, int32_t rank, int32_t world, uint64_t slot_bytes, uint8_t* blob_out) { ENTER(ctx);
   CHECK_ARG(blob_out != nullptr, "comm_create: blob_out is NULL");
+  CHECK_ARG(world >= 1 && world <= DBSP_COMM_MAX_RANKS, "comm_create: world = " + std::to_string(world) + ": 1..32 ranks");
+  CHECK_ARG(rank >= 0 && rank < world, "comm_create: rank = " + std::to_string(rank) + " is not below world = " + std::to_string(world));
   return comm_create(ctx, rank, world, slot_bytes, blob_out);
 }
 int32_t dbsp_comm_connect(dbsp_ctx* ctx, const uint8_t* blobs) { ENTER(ctx);
@@ -1108,6 +1342,7 @@ int32_t dbsp_comm_destroy(dbsp_ctx* ctx) { ENTER(ctx);
   return DBSP_OK;
 }
 int32_t dbsp_comm_info(dbsp_ctx* ctx, int32_t* rank, int32_t* world, uint64_t* bytes_sent) {
+  NOT_NULL(ctx, "ctx");
   int r, w;
   u64 b;
   comm_info(ctx, &r, &w, &b);
@@ -1117,6 +1352,8 @@ int32_t dbsp_comm_info(dbsp_ctx* ctx, int32_t* rank, int32_t* world, uint64_t* b
   return DBSP_OK;
 }
 int32_t dbsp_shard(dbsp_ctx* ctx, const dbsp_batch* b, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
   const Batch* in[1] = {B(b)};
   Batch* o[1] = {nullptr};
   TRY(comm_exchange(ctx, in, 1, -1, o));
@@ -1124,6 +1361,10 @@ int32_t dbsp_shard(dbsp_ctx* ctx, const dbsp_batch* b, dbsp_batch** out) { ENTER
   return DBSP_OK;
 }
 int32_t dbsp_shard2(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b, dbsp_batch** out_a, dbsp_batch** out_b) { ENTER(ctx);
+  NOT_NULL(out_a, "out_a");
+  NOT_NULL(out_b, "out_b");
+  NOT_NULL(a, "a");
+  NOT_NULL(b, "b");
   const Batch* in[2] = {B(a), B(b)};
   Batch* o[2] = {nullptr, nullptr};
   TRY(comm_exchange(ctx, in, 2, -1, o));
@@ -1132,9 +1373,11 @@ int32_t dbsp_shard2(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b, dbs
   return DBSP_OK;
 }
 int32_t dbsp_gather(dbsp_ctx* ctx, const dbsp_batch* b, int32_t root, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
   int r, w;
   comm_info(ctx, &r, &w, nullptr);
-  CHECK_ARG(root >= 0 && root < w, "gather: root out of range");
+  CHECK_ARG(root >= 0 && root < w, "gather: root = " + std::to_string(root) + " is not a rank of a group of " + std::to_string(w));
   const Batch* in[1] = {B(b)};
   Batch* o[1] = {nullptr};
   TRY(comm_exchange(ctx, in, 1, root, o));
@@ -1142,6 +1385,7 @@ int32_t dbsp_gather(dbsp_ctx* ctx, const dbsp_batch* b, int32_t root, dbsp_batch
   return DBSP_OK;
 }
 int32_t dbsp_allreduce_max_u64(dbsp_ctx* ctx, uint64_t* x) { ENTER(ctx);
+  NOT_NULL(x, "x");
   u64 v = *x;
   TRY(comm_allreduce_max(ctx, &v));
   *x = v;

@@ -295,8 +295,8 @@ int32_t comm_create(Ctx* ctx, int rank, int world, u64 slot_bytes, unsigned char
   c->region_bytes = CTRL_BYTES + (size_t)2 * world * c->slot_bytes;
   cudaError_t e = cudaMalloc(&c->region, c->region_bytes);
   if (e != cudaSuccess) {
-    delete c;
     set_error(std::string("comm_create: cudaMalloc of the receive region (") + std::to_string(c->region_bytes) + " B): " + cudaGetErrorString(e));
+    delete c;
     return DBSP_ERR_CUDA;
   }
   ctx->comm = c;

@@ -207,6 +207,11 @@ void comm_info(Ctx* ctx, int* rank, int* world, u64* bytes_sent);
 int32_t consolidate_rows(Ctx* ctx, const dbsp_schema& s, const Cols& cols, const i64* w, u64 n, const BufP* adopt,
                          Batch** out, const u32* d_n = nullptr);
 
+// The census consolidate_rows starts with, on its own: rows i-1 > i, rows i-1 == i, weights == 0 (one launch pair,
+// one read-back).  All three are zero exactly when the rows are a canonical batch.
+int32_t rows_census(Ctx* ctx, const dbsp_schema& s, const Cols& cols, const i64* w, u64 n, u64* inversions, u64* duplicates,
+                    u64* zero_weights);
+
 int32_t reduce_sorted_rows(Ctx* ctx, const dbsp_schema& s, const Cols& cols, const i64* w, u64 n, Batch** out);
 
 // ---- merge.cu --------------------------------------------------------------

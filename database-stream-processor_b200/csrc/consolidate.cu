@@ -483,6 +483,51 @@ inline int bits_for(u64 range) { return range == 0 ? 0 : 64 - __builtin_clzll(ra
 int32_t radix_sort_pairs(Ctx* ctx, int words, u64* k0a, u64* k0b, u64* k1a, u64* k1b, u32* ida, u32* idb, u64 n, int bits_lo, int bits_hi,
                          int presorted_top_bits, bool force_lsd, unsigned long long* fail, int* which, int* hbm_passes);
 
+// Lane ranges + order / duplicate / zero-weight census of n > 0 rows: one launch pair and one read-back (the layout
+// of mm is k_props').
+static int32_t census(Ctx* ctx, int L, const Cols& cols, const Flips& f, const i64* w, u64 n, const u32* d_n, u64* mm) {
+  cudaStream_t st = ctx->stream;
+  const int TB = 256;
+  u64* dmm = ctx->d_scratch + 64;
+  k_init_props<<<1, 32, 0, st>>>(dmm, L);
+  const Mail mail = mail_begin(ctx);
+  int g = (int)std::min<u64>((n + TB - 1) / TB, (u64)ctx->sm_count * 8);
+  {
+    ProfScope ps(ctx, KID_MINMAX, n * (u64)(L + (w ? 1 : 0)) * 8);
+    switch (L) {
+      case 1: k_props<1><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
+      case 2: k_props<2><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
+      case 3: k_props<3><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
+      case 4: k_props<4><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
+      case 5: k_props<5><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
+      case 6: k_props<6><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
+      case 7: k_props<7><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
+      default: k_props<8><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
+    }
+  }
+  ctx->kernel_launches += 2;
+  return mail_finish(ctx, mail, mm, 2 * L + 6);
+}
+
+static Flips schema_flips(const dbsp_schema& s) {
+  const int L = s.n_key_lanes + s.n_val_lanes;
+  Flips f;
+  for (int l = 0; l < MAXL; l++) f.f[l] = (l < L && s.lane_types[l] == DBSP_I64) ? 0x8000000000000000ull : 0;
+  return f;
+}
+
+int32_t rows_census(Ctx* ctx, const dbsp_schema& s, const Cols& cols, const i64* w, u64 n, u64* inversions, u64* duplicates, u64* zero_weights) {
+  *inversions = *duplicates = *zero_weights = 0;
+  if (n == 0) return DBSP_OK;
+  const int L = s.n_key_lanes + s.n_val_lanes;
+  u64 mm[2 * MAXL + 6];
+  TRY(census(ctx, L, cols, schema_flips(s), w, n, nullptr, mm));
+  *inversions = mm[2 * L];
+  *duplicates = mm[2 * L + 1];
+  *zero_weights = mm[2 * L + 2];
+  return DBSP_OK;
+}
+
 int32_t consolidate_rows(Ctx* ctx, const dbsp_schema& s, const Cols& cols, const i64* w, u64 n, const BufP* adopt,
                          Batch** out, const u32* d_n) {
   const int L = s.n_key_lanes + s.n_val_lanes;
@@ -491,35 +536,14 @@ int32_t consolidate_rows(Ctx* ctx, const dbsp_schema& s, const Cols& cols, const
   cudaStream_t st = ctx->stream;
   const int TB = 256;
 
-  Flips f;
-  for (int l = 0; l < MAXL; l++) f.f[l] = (l < L && s.lane_types[l] == DBSP_I64) ? 0x8000000000000000ull : 0;
+  const Flips f = schema_flips(s);
 
   // ---- (1) lane ranges + order / duplicate / zero-weight census ---------------
   u64 mm[2 * MAXL + 6];
-  {
-    u64* dmm = ctx->d_scratch + 64;
-    k_init_props<<<1, 32, 0, st>>>(dmm, L);
-    const Mail mail = mail_begin(ctx);
-    int g = (int)std::min<u64>((n + TB - 1) / TB, (u64)ctx->sm_count * 8);
-    {
-      ProfScope ps(ctx, KID_MINMAX, n * (u64)(L + (w ? 1 : 0)) * 8);
-      switch (L) {
-        case 1: k_props<1><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
-        case 2: k_props<2><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
-        case 3: k_props<3><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
-        case 4: k_props<4><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
-        case 5: k_props<5><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
-        case 6: k_props<6><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
-        case 7: k_props<7><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
-        default: k_props<8><<<g, TB, 0, st>>>(cols, f, w, n, d_n, dmm, mail); break;
-      }
-    }
-    ctx->kernel_launches += 2;
-    TRY(mail_finish(ctx, mail, mm, 2 * L + 6));
-    if (d_n) {
-      n = mm[2 * L + 3];
-      if (n == 0) { *out = batch_new_empty(ctx, s); return DBSP_OK; }
-    }
+  TRY(census(ctx, L, cols, f, w, n, d_n, mm));
+  if (d_n) {
+    n = mm[2 * L + 3];
+    if (n == 0) { *out = batch_new_empty(ctx, s); return DBSP_OK; }
   }
   const unsigned nblk = (unsigned)((n + TB - 1) / TB);
   const u64 n_inv = mm[2 * L], n_dup = mm[2 * L + 1], n_zero = mm[2 * L + 2];

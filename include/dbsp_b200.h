@@ -15,7 +15,20 @@
  *     replica to its worker thread, circuit_builder.rs:1439-1450);
  *   - batches are immutable, reference counted values (the reference's
  *     batches are immutable values too, zset_batch.rs:27);
- *   - every *_free is a no-op on NULL.
+ *   - every *_free (and dbsp_download_finish) is a no-op on NULL.
+ *
+ * Error contract.  Every argument is checked on the host before the call
+ * allocates, copies or launches anything.  A refused call returns
+ * DBSP_ERR_INVALID (DBSP_ERR_UNSUPPORTED for 2^32-1 or more rows in one
+ * batch), leaves a dbsp_last_error text naming the call and the argument,
+ * writes no out-pointer and leaves the context and its handles usable.
+ * Refused everywhere: a NULL context, a NULL handle, a NULL in- or out-pointer
+ * that a comment below does not call optional; a schema without 1..8 lanes
+ * or with a lane type other than DBSP_U64 / DBSP_I64; a row expression whose
+ * kind / op / cmp is outside its enum, whose n_pred exceeds DBSP_MAX_PREDS or
+ * whose idx is not below the lane count of the source it names; two operands
+ * whose schemas do not fit each other (noted per call).  DESIGN.md §1 lists
+ * the checks of every entry point.
  *
  * Data model.  A row is `n_key_lanes + n_val_lanes` 64-bit lanes plus one
  * int64 weight.  Lanes are u64 or i64 and compare lexicographically, which
@@ -65,7 +78,8 @@ enum dbsp_src_kind {
   DBSP_SRC_KEY = 0,   /* lane `idx` of the (join) key                       */
   DBSP_SRC_LVAL = 1,  /* lane `idx` of the left value (v1 of join_func);
                          for map_index / raw tables: value lane / column    */
-  DBSP_SRC_RVAL = 2,  /* lane `idx` of the right value (v2 of join_func)    */
+  DBSP_SRC_RVAL = 2,  /* lane `idx` of the right value (v2 of join_func);
+                         in a call with one input: the same lanes as LVAL  */
   DBSP_SRC_CONST = 3  /* the constant `cst`                                 */
 };
 enum dbsp_expr_op {
@@ -166,7 +180,8 @@ int32_t dbsp_batch_from_tuples(dbsp_ctx* ctx, const dbsp_schema* schema,
                                const int64_t* weights, uint64_t n,
                                int32_t on_device, dbsp_batch** out);
 /* flat_map_index over a raw (unsorted, column-major) event table followed by
- * from_tuples (filter_map.rs:700-724): SRC_LVAL idx = column index. */
+ * from_tuples (filter_map.rs:700-724): every source kind names a column,
+ * idx < n_cols (1..8).  Only the columns `proj` reads need be non-NULL. */
 int32_t dbsp_batch_from_table(dbsp_ctx* ctx, const uint64_t* const* cols,
                               uint32_t n_cols, const int64_t* weights,
                               uint64_t n, int32_t on_device,
@@ -176,7 +191,8 @@ int32_t dbsp_batch_from_table(dbsp_ctx* ctx, const uint64_t* const* cols,
  * memory makes it overlap with the kernels of the current step); the handle
  * is then consumed by dbsp_batch_from_upload.  `col_mask` bit l = column l is
  * needed (the others are not copied).  The host buffers must stay valid until
- * the upload is consumed or freed.  This is the double-buffered input queue of
+ * the upload is consumed or freed.  dbsp_batch_from_upload refuses a `proj`
+ * that reads a column outside `col_mask`.  This is the double-buffered input queue of
  * the reference's source operators (crates/nexmark/src/lib.rs:105-231 feeds
  * batches ahead of the circuit) moved to the PCIe boundary. */
 typedef struct dbsp_upload dbsp_upload;
@@ -187,7 +203,8 @@ int32_t dbsp_upload_begin(dbsp_ctx* ctx, const uint64_t* const* cols,
 int32_t dbsp_batch_from_upload(dbsp_ctx* ctx, dbsp_upload* up,
                                const dbsp_proj* proj, dbsp_batch** out);
 int32_t dbsp_upload_free(dbsp_upload* up);
-/* Columns of the table a projection reads (bit l = SRC_LVAL idx l). */
+/* Columns of the table a projection reads (bit l = a source with idx l);
+ * 0 for a NULL or malformed projection.  Needs no context. */
 uint32_t dbsp_proj_table_mask(const dbsp_proj* proj);
 int32_t dbsp_batch_empty(dbsp_ctx* ctx, const dbsp_schema* schema,
                          dbsp_batch** out);
@@ -226,7 +243,10 @@ int32_t dbsp_batch_merge_bounded(dbsp_ctx* ctx, const dbsp_batch* a,
 /* The fuelled Merger (trace/mod.rs:371-396: new_merger / work / done).
  * work() spends at most *fuel units (here: input rows) and subtracts what it
  * used; *fuel > 0 after the call <=> the merge is complete (:388-395).
- * done() requires a complete merge, returns the batch and frees the merger. */
+ * *fuel <= 0 is not an error: no work is done and *fuel comes back unchanged
+ * (as 1 when the merge is already complete).  done() requires a complete
+ * merge (else DBSP_ERR_INVALID and the merger stays the caller's), returns
+ * the batch and frees the merger.  a and b must have one schema. */
 typedef struct dbsp_merger dbsp_merger;
 int32_t dbsp_merger_new(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b,
                         const uint64_t* val_lower_bound, dbsp_merger** out);
@@ -312,7 +332,11 @@ int32_t dbsp_spine_free(dbsp_spine* s);
  * PersistentTrace (crates/dbsp/src/trace/persistent/) for snapshots.  One little-endian file: magic "DBSPSPN1",
  * the schema, key / value bounds, effort, then every layer of the spine (spine_fueled.rs:1012-1027: Vacant /
  * Single / Double{InProgress, Complete}) with its batches as flat lanes + weights and, for a merge in progress,
- * the fuel still owed — so a loaded spine resumes the same merge schedule.  The format is shared with the oracle. */
+ * the fuel still owed — so a loaded spine resumes the same merge schedule.  The format is shared with the oracle.
+ * dbsp_spine_load treats the file as outside input: every field is checked as it is read and before anything is
+ * allocated for it (schema, flags, layer count and kinds, which batches a layer may hold, row counts against the
+ * bytes left, the fuel owed, no trailing bytes), and the rows of every batch must be ordered, free of duplicate rows
+ * and of zero weights; otherwise DBSP_ERR_INVALID, and everything already loaded is freed. */
 int32_t dbsp_spine_save(dbsp_ctx* ctx, const dbsp_spine* s, const char* path);
 int32_t dbsp_spine_load(dbsp_ctx* ctx, const char* path, dbsp_spine** out);
 
@@ -324,11 +348,14 @@ int32_t dbsp_spine_load(dbsp_ctx* ctx, const char* path, dbsp_spine** out);
 int32_t dbsp_join_delta_trace(dbsp_ctx* ctx, const dbsp_batch* delta,
                               const dbsp_spine* trace, const dbsp_proj* proj,
                               int32_t delta_is_left, dbsp_batch** out);
-/* Join::eval (join.rs:436-473): stateless batch x batch. */
+/* Join::eval (join.rs:436-473): stateless batch x batch.  Both joins need
+ * equal key lanes (count and types) on the two sides; `proj` may name the key
+ * lanes, the left side's value lanes (LVAL) and the right side's (RVAL). */
 int32_t dbsp_join_batches(dbsp_ctx* ctx, const dbsp_batch* left,
                           const dbsp_batch* right, const dbsp_proj* proj,
                           dbsp_batch** out);
-/* SemiJoinStream::eval (operator/semijoin.rs:100-142). */
+/* SemiJoinStream::eval (operator/semijoin.rs:100-142).  `keys` has the key
+ * lanes of `pairs` and no value lanes. */
 int32_t dbsp_semijoin(dbsp_ctx* ctx, const dbsp_batch* pairs,
                       const dbsp_batch* keys, dbsp_batch** out);
 /* AggregateIncremental::eval (aggregate/mod.rs:600-684) fused with
@@ -336,15 +363,20 @@ int32_t dbsp_semijoin(dbsp_ctx* ctx, const dbsp_batch* pairs,
  * aggregate the key's values in `in_trace` (which already contains delta),
  * compare with the key's current value in `out_trace`, emit -1/+1 rows.
  * The caller then inserts *out into out_trace (the TraceAppend of
- * upsert.rs:69-107). */
+ * upsert.rs:69-107).  delta and in_trace have one schema; out_trace has their
+ * key lanes (WCOUNT2: all but the last) and the values of the aggregator:
+ * MAX / MIN the input's values (at least one lane), FOLD_* one lane over an
+ * input with values, WCOUNT one lane and WCOUNT2 two over an input without. */
 int32_t dbsp_aggregate_delta(dbsp_ctx* ctx, const dbsp_batch* delta,
                              const dbsp_spine* in_trace,
                              const dbsp_spine* out_trace, int32_t agg_kind,
                              dbsp_batch** out);
-/* weigh (aggregate/mod.rs:297-323). `f` gives f(k,v) (SRC_KEY/SRC_LVAL). */
+/* weigh (aggregate/mod.rs:297-323). `f` gives f(k,v) (SRC_KEY/SRC_LVAL).
+ * `mode` is a dbsp_weigh_mode; WEIGH_AVG adds a key lane (at most 7 before). */
 int32_t dbsp_weigh(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_expr* f,
                    int32_t mode, dbsp_batch** out);
-/* DistinctIncrementalTotal::eval (operator/distinct.rs:196-254). */
+/* DistinctIncrementalTotal::eval (operator/distinct.rs:196-254).  delta and
+ * the integral have one schema. */
 int32_t dbsp_distinct_delta(dbsp_ctx* ctx, const dbsp_batch* delta,
                             const dbsp_spine* delayed_integral,
                             dbsp_batch** out);
@@ -352,7 +384,8 @@ int32_t dbsp_distinct_delta(dbsp_ctx* ctx, const dbsp_batch* delta,
 int32_t dbsp_stream_distinct(dbsp_ctx* ctx, const dbsp_batch* b,
                              dbsp_batch** out);
 /* Window::eval (operator/time_series/window.rs:144-222).  Bounds are
- * n_key_lanes u64 each; has_prev == 0 on the first step. */
+ * n_key_lanes u64 each; has_prev == 0 on the first step (start0 / end0 may
+ * then be NULL).  trace and delta have one schema. */
 int32_t dbsp_window_delta(dbsp_ctx* ctx, const dbsp_spine* trace,
                           const dbsp_batch* delta, int32_t has_prev,
                           const uint64_t* start0, const uint64_t* end0,
@@ -362,7 +395,7 @@ int32_t dbsp_window_delta(dbsp_ctx* ctx, const dbsp_spine* trace,
 int32_t dbsp_map_index(dbsp_ctx* ctx, const dbsp_batch* b,
                        const dbsp_proj* proj, dbsp_batch** out);
 /* shard_batch (operator/communication/shard.rs:165-199): split by
- * hash(key) % n_shards into n_shards ordered batches.  The exchange itself
+ * hash(key) % n_shards into n_shards (1..64) ordered batches.  The exchange itself
  * (exchange.rs:128-200) is done by the host with its collective library on
  * dbsp_batch_device_columns(); the receiver merges (shard.rs:136-144). */
 int32_t dbsp_shard_partition(dbsp_ctx* ctx, const dbsp_batch* b,
@@ -400,7 +433,8 @@ int32_t dbsp_gather(dbsp_ctx* ctx, const dbsp_batch* b, int32_t root, dbsp_batch
 int32_t dbsp_allreduce_max_u64(dbsp_ctx* ctx, uint64_t* x);
 
 /* Builder path (trace/mod.rs:338-368): adopt rows that are already sorted
- * and consolidated (e.g. a segment received from a peer). */
+ * and consolidated (e.g. a segment received from a peer).  `weights` is
+ * required; the rows are taken on trust. */
 int32_t dbsp_batch_from_sorted(dbsp_ctx* ctx, const dbsp_schema* schema,
                                const uint64_t* const* cols,
                                const int64_t* weights, uint64_t n,

@@ -28,6 +28,7 @@
 #include <vector>
 
 #include "../include/dbsp_b200.h"
+#include "../database-stream-processor_b200/csrc/validate.h"
 
 typedef uint64_t u64;
 typedef int64_t i64;
@@ -722,60 +723,132 @@ static thread_local std::string g_err;
 
 static orc_batch* wrap(BatchP p) { return new orc_batch{p}; }
 
+// The error contract of include/dbsp_b200.h, with the CUDA library's rules and texts (validate.h): every argument is
+// checked before the call reads or builds anything.  WHAT is the call's name without the prefix.
+namespace dv = dbsp_validate;
+#define CHECK_ARG(c, msg)                                  \
+  do {                                                     \
+    if (!(c)) { g_err = (msg); return DBSP_ERR_INVALID; } \
+  } while (0)
+#define WHAT (__func__ + 4)
+#define NOT_NULL(p, name) CHECK_ARG((p) != nullptr, std::string(WHAT) + ": " name " is NULL")
+#define REFUSE(text)                                               \
+  do {                                                             \
+    const std::string m__ = (text);                                \
+    if (!m__.empty()) { g_err = m__; return DBSP_ERR_INVALID; }   \
+  } while (0)
+#define ROWS32(n)                                                                                \
+  do {                                                                                           \
+    if ((u64)(n) >= 0xffffffffull) {                                                             \
+      g_err = std::string(WHAT) + ": n = " + std::to_string(n) + ": 2^32-1 or more rows in one batch; split the batch"; \
+      return DBSP_ERR_UNSUPPORTED;                                                               \
+    }                                                                                            \
+  } while (0)
+static std::string valid_cols(const char* what, const u64* const* cols, int ncols, u64 n, unsigned mask = ~0u) {
+  if (!cols) return std::string(what) + ": cols is NULL";
+  for (int l = 0; n && l < ncols; l++)
+    if (((mask >> l) & 1) && !cols[l]) return std::string(what) + ": cols[" + std::to_string(l) + "] is NULL";
+  return "";
+}
+static std::string valid_join(const char* what, const dbsp_schema& left, const dbsp_schema& right, const dbsp_proj* p) {
+  if (!dv::same_key_lanes(left, right)) return std::string(what) + ": the two inputs differ in key lanes (count or type)";
+  return dv::valid_proj(p, left.n_key_lanes, left.n_val_lanes, right.n_val_lanes, what);
+}
+
 extern "C" {
 
-int32_t orc_ctx_create(int32_t, orc_ctx** out) { *out = new orc_ctx{0}; return DBSP_OK; }
+int32_t orc_ctx_create(int32_t device, orc_ctx** out) {
+  NOT_NULL(out, "out");
+  CHECK_ARG(device >= 0, "ctx_create: device is negative");
+  *out = new orc_ctx{0};
+  return DBSP_OK;
+}
 int32_t orc_ctx_destroy(orc_ctx* c) { delete c; return DBSP_OK; }
-int32_t orc_ctx_sync(orc_ctx*) { return DBSP_OK; }
+int32_t orc_ctx_sync(orc_ctx* c) { NOT_NULL(c, "ctx"); return DBSP_OK; }
 const char* orc_last_error(void) { return g_err.c_str(); }
-int32_t orc_ctx_stats(orc_ctx*, u64* a, u64* b, u64* c, int32_t) { if (a) *a = 0; if (b) *b = 0; if (c) *c = 0; return DBSP_OK; }
+int32_t orc_ctx_stats(orc_ctx* ctx, u64* a, u64* b, u64* c, int32_t) { NOT_NULL(ctx, "ctx"); if (a) *a = 0; if (b) *b = 0; if (c) *c = 0; return DBSP_OK; }
 void* orc_ctx_stream(orc_ctx*) { return nullptr; }
-int32_t orc_ctx_profile(orc_ctx*, int32_t) { return DBSP_OK; }
+int32_t orc_ctx_profile(orc_ctx* c, int32_t) { NOT_NULL(c, "ctx"); return DBSP_OK; }
 int32_t orc_ctx_profile_read(orc_ctx*, int32_t, char*, u64*, double*, u64*) { return DBSP_ERR_INVALID; }
 
-int32_t orc_batch_from_tuples(orc_ctx*, const dbsp_schema* s, const u64* const* cols, const i64* w, u64 n,
+int32_t orc_batch_from_tuples(orc_ctx* c, const dbsp_schema* s, const u64* const* cols, const i64* w, u64 n,
                               int32_t, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_schema(s, WHAT));
+  REFUSE(valid_cols(WHAT, cols, s->n_key_lanes + s->n_val_lanes, n));
+  ROWS32(n);
   *out = wrap(from_tuples(*s, cols, w, n));
   return DBSP_OK;
 }
 
 // FlatMap::eval + from_tuples (operator/filter_map.rs:700-724).
-int32_t orc_batch_from_table(orc_ctx*, const u64* const* cols, uint32_t ncols, const i64* w, u64 n, int32_t,
-                             const dbsp_proj* proj, orc_batch** out) {
+static int32_t table_to_batch(const char* what, const u64* const* cols, uint32_t ncols, unsigned col_mask, const i64* w, u64 n,
+                              const dbsp_proj* proj, orc_batch** out) {
+  REFUSE(dv::valid_proj(proj, (int)ncols, (int)ncols, (int)ncols, what));
+  const unsigned used = dv::proj_table_mask(*proj);
+  CHECK_ARG((used & ~col_mask) == 0, std::string(what) + ": proj reads column " + std::to_string(__builtin_ctz((used & ~col_mask) | 0x100u)) +
+                                         ", which col_mask left out of the upload");
+  REFUSE(valid_cols(what, cols, (int)ncols, n, used));
   Tuples t(proj->out_schema);
   u64 lv[MAXL] = {0}, row[MAXL];
   for (u64 i = 0; i < n; i++) {
-    for (uint32_t c = 0; c < ncols && c < MAXL; c++) lv[c] = cols[c][i];
+    for (uint32_t c = 0; c < ncols; c++) if ((used >> c) & 1) lv[c] = cols[c][i];
     Env e{lv, lv, lv};
     if (project(*proj, e, row)) t.push(row, w ? w[i] : 1);
   }
   *out = wrap(t.build());
   return DBSP_OK;
 }
+int32_t orc_batch_from_table(orc_ctx* c, const u64* const* cols, uint32_t ncols, const i64* w, u64 n, int32_t,
+                             const dbsp_proj* proj, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  CHECK_ARG(ncols >= 1 && ncols <= MAXL, "batch_from_table: n_cols = " + std::to_string(ncols) + ": a table has 1..8 columns");
+  ROWS32(n);
+  return table_to_batch(WHAT, cols, ncols, ~0u, w, n, proj, out);
+}
 
 // pipelined ingest: on the CPU there is nothing to overlap, keep the pointers
-struct orc_upload { const u64* const* cols; uint32_t n_cols; const i64* w; u64 n; std::vector<const u64*> own; };
-int32_t orc_batch_from_table(orc_ctx*, const u64* const* cols, uint32_t ncols, const i64* w, u64 n, int32_t,
-                             const dbsp_proj* proj, orc_batch** out);
-int32_t orc_upload_begin(orc_ctx*, const u64* const* cols, uint32_t n_cols, uint32_t, const i64* w, u64 n, orc_upload** out) {
+struct orc_upload { const u64* const* cols; uint32_t n_cols; uint32_t col_mask; const i64* w; u64 n; std::vector<const u64*> own; };
+int32_t orc_upload_begin(orc_ctx* c, const u64* const* cols, uint32_t n_cols, uint32_t col_mask, const i64* w, u64 n, orc_upload** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "upload_begin: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
+  REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, col_mask));
+  ROWS32(n);
   orc_upload* u = new orc_upload();
   u->own.assign(cols, cols + n_cols);
-  u->cols = u->own.data(); u->n_cols = n_cols; u->w = w; u->n = n;
+  u->cols = u->own.data(); u->n_cols = n_cols; u->col_mask = col_mask; u->w = w; u->n = n;
   *out = u;
   return DBSP_OK;
 }
 int32_t orc_batch_from_upload(orc_ctx* c, orc_upload* u, const dbsp_proj* proj, orc_batch** out) {
-  return orc_batch_from_table(c, u->cols, u->n_cols, u->w, u->n, 0, proj, out);
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(u, "upload");
+  return table_to_batch(WHAT, u->cols, u->n_cols, u->col_mask, u->w, u->n, proj, out);
 }
 int32_t orc_upload_free(orc_upload* u) { delete u; return DBSP_OK; }
-uint32_t orc_proj_table_mask(const dbsp_proj*) { return 0xffu; }
+uint32_t orc_proj_table_mask(const dbsp_proj* proj) {
+  if (!dv::valid_proj(proj, MAXL, MAXL, MAXL, "proj_table_mask").empty()) return 0;
+  return dv::proj_table_mask(*proj);
+}
 
-int32_t orc_batch_empty(orc_ctx*, const dbsp_schema* s, orc_batch** out) {
+int32_t orc_batch_empty(orc_ctx* c, const dbsp_schema* s, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_schema(s, WHAT));
   *out = wrap(std::make_shared<Batch>(*s));
   return DBSP_OK;
 }
 
-int32_t orc_batch_merge(orc_ctx*, const orc_batch* a, const orc_batch* b, orc_batch** out) {
+int32_t orc_batch_merge(orc_ctx* c, const orc_batch* a, const orc_batch* b, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(a, "a");
+  NOT_NULL(b, "b");
+  CHECK_ARG(dv::same_schema(a->p->s, b->p->s), std::string(WHAT) + ": a and b differ in schema");
   *out = wrap(merge(a->p, b->p));
   return DBSP_OK;
 }
@@ -795,15 +868,30 @@ static void batcher_enqueue(orc_batcher* q, BatchP b) {
     if (m->len()) q->queue.push_back(m);
   }
 }
-int32_t orc_batcher_new(orc_ctx*, const dbsp_schema* s, orc_batcher** out) { *out = new orc_batcher{*s, {}}; return DBSP_OK; }
-int32_t orc_batcher_push(orc_ctx*, orc_batcher* q, const u64* const* cols, const i64* w, u64 n, int32_t) {
+int32_t orc_batcher_new(orc_ctx* c, const dbsp_schema* s, orc_batcher** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_schema(s, WHAT));
+  *out = new orc_batcher{*s, {}};
+  return DBSP_OK;
+}
+int32_t orc_batcher_push(orc_ctx* c, orc_batcher* q, const u64* const* cols, const i64* w, u64 n, int32_t) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(q, "batcher");
+  REFUSE(valid_cols(WHAT, cols, q->s.n_key_lanes + q->s.n_val_lanes, n));
+  ROWS32(n);
   if (n) batcher_enqueue(q, from_tuples(q->s, cols, w, n));
   return DBSP_OK;
 }
 int32_t orc_batch_from_sorted(orc_ctx* c, const dbsp_schema* s, const u64* const* cols, const i64* w, u64 n, int32_t od,
                               orc_batch** out);
 int32_t orc_batcher_push_consolidated(orc_ctx* c, orc_batcher* q, const u64* const* cols, const i64* w, u64 n, int32_t od) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(q, "batcher");
+  REFUSE(valid_cols(WHAT, cols, q->s.n_key_lanes + q->s.n_val_lanes, n));
+  ROWS32(n);
   if (!n) return DBSP_OK;
+  CHECK_ARG(w != nullptr, "batcher_push_consolidated: weights is NULL (consolidated rows carry their weights)");
   orc_batch* b = nullptr;
   int32_t rc = orc_batch_from_sorted(c, &q->s, cols, w, n, od, &b);
   if (rc) return rc;
@@ -811,9 +899,12 @@ int32_t orc_batcher_push_consolidated(orc_ctx* c, orc_batcher* q, const u64* con
   delete b;
   return DBSP_OK;
 }
-int32_t orc_batcher_tuples(const orc_batcher* q, u64* n) { u64 t = 0; for (auto& b : q->queue) t += b->len(); *n = t; return DBSP_OK; }
+int32_t orc_batcher_tuples(const orc_batcher* q, u64* n) { NOT_NULL(q, "batcher"); NOT_NULL(n, "n_tuples"); u64 t = 0; for (auto& b : q->queue) t += b->len(); *n = t; return DBSP_OK; }
 int32_t orc_batcher_free(orc_batcher* q) { delete q; return DBSP_OK; }
-int32_t orc_batcher_seal(orc_ctx*, orc_batcher* q, orc_batch** out) {
+int32_t orc_batcher_seal(orc_ctx* c, orc_batcher* q, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(q, "batcher");
+  NOT_NULL(out, "out");
   while (q->queue.size() >= 2) {
     BatchP y = q->queue.back(); q->queue.pop_back();
     BatchP x = q->queue.back(); q->queue.pop_back();
@@ -828,42 +919,63 @@ int32_t orc_batcher_seal(orc_ctx*, orc_batcher* q, orc_batch** out) {
 // Merger::work with a lower value bound run to completion
 // (indexed_zset_batch.rs:359-382; ordered/mod.rs:587-746).  OrdZSet ignores the
 // bound (zset_batch.rs:307-318).
-int32_t orc_batch_merge_bounded(orc_ctx*, const orc_batch* a, const orc_batch* b, const u64* vb, orc_batch** out) {
-  if (memcmp(&a->p->s, &b->p->s, sizeof(dbsp_schema))) { g_err = "merge: schema mismatch"; return DBSP_ERR_INVALID; }
+int32_t orc_batch_merge_bounded(orc_ctx* c, const orc_batch* a, const orc_batch* b, const u64* vb, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(a, "a");
+  NOT_NULL(b, "b");
+  CHECK_ARG(dv::same_schema(a->p->s, b->p->s), std::string(WHAT) + ": a and b differ in schema");
   *out = wrap(merge(a->p, b->p, a->p->indexed() ? vb : nullptr));
   return DBSP_OK;
 }
 struct orc_merger { Merger m; bool has_vb; u64 vb[MAXL]; };
-int32_t orc_merger_new(orc_ctx*, const orc_batch* a, const orc_batch* b, const u64* vb, orc_merger** out) {
-  if (memcmp(&a->p->s, &b->p->s, sizeof(dbsp_schema))) { g_err = "merger: schema mismatch"; return DBSP_ERR_INVALID; }
+int32_t orc_merger_new(orc_ctx* c, const orc_batch* a, const orc_batch* b, const u64* vb, orc_merger** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(a, "a");
+  NOT_NULL(b, "b");
+  CHECK_ARG(dv::same_schema(a->p->s, b->p->s), std::string(WHAT) + ": a and b differ in schema");
   orc_merger* m = new orc_merger{Merger(a->p, b->p), vb != nullptr && a->p->indexed(), {0}};
   if (m->has_vb) for (int l = 0; l < a->p->s.n_val_lanes; l++) m->vb[l] = vb[l];
   *out = m;
   return DBSP_OK;
 }
-int32_t orc_merger_work(orc_ctx*, orc_merger* m, i64* fuel) {
+int32_t orc_merger_work(orc_ctx* c, orc_merger* m, i64* fuel) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(m, "merger");
+  NOT_NULL(fuel, "fuel");
   if (m->m.complete()) { *fuel = std::max<i64>(*fuel, 1); return DBSP_OK; }
   if (*fuel > 0) m->m.work(m->has_vb ? m->vb : nullptr, fuel);
   if (m->m.complete()) *fuel = std::max<i64>(*fuel, 1);   // ABI: fuel > 0 after the call <=> merge complete
   else *fuel = std::min<i64>(*fuel, 0);
   return DBSP_OK;
 }
-int32_t orc_merger_done(orc_ctx*, orc_merger* m, orc_batch** out) {
-  if (!m->m.complete()) { g_err = "merger_done: merge not complete"; return DBSP_ERR_INVALID; }
+int32_t orc_merger_done(orc_ctx* c, orc_merger* m, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(m, "merger");
+  NOT_NULL(out, "out");
+  CHECK_ARG(m->m.complete(), "merger_done: merger: the merge is not complete (merger_work left fuel <= 0)");
   *out = wrap(m->m.out);
   delete m;
   return DBSP_OK;
 }
 int32_t orc_merger_free(orc_merger* m) { delete m; return DBSP_OK; }
 // BatchReader::truncate_keys_below (trace/mod.rs:227-233).
-int32_t orc_batch_truncate_keys_below(orc_ctx*, const orc_batch* b, const u64* key, orc_batch** out) {
+int32_t orc_batch_truncate_keys_below(orc_ctx* c, const orc_batch* b, const u64* key, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  CHECK_ARG(key != nullptr || b->p->s.n_key_lanes == 0, "batch_truncate_keys_below: key is NULL");
   BatchP t = truncate_keys_below(*b->p, key);
   *out = wrap(t ? t : b->p);
   return DBSP_OK;
 }
 
 // neg (column_layer/mod.rs:452-480).
-int32_t orc_batch_neg(orc_ctx*, const orc_batch* a, orc_batch** out) {
+int32_t orc_batch_neg(orc_ctx* c, const orc_batch* a, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(a, "batch");
   auto o = std::make_shared<Batch>(*a->p);
   for (auto& x : o->w) x = (i64)((u64)0 - (u64)x);
   *out = wrap(o);
@@ -885,10 +997,13 @@ static void flat_rows(const Batch& b, Tuples& t) {
 }
 
 // index() (operator/index.rs:128-157) and its inverse: re-split the lanes.
-int32_t orc_batch_reindex(orc_ctx*, const orc_batch* a, uint32_t nk, orc_batch** out) {
+int32_t orc_batch_reindex(orc_ctx* c, const orc_batch* a, uint32_t nk, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(a, "batch");
   dbsp_schema s = a->p->s;
   int nl = s.n_key_lanes + s.n_val_lanes;
-  if ((int)nk > nl) return DBSP_ERR_INVALID;
+  CHECK_ARG(nk <= (uint32_t)nl, "batch_reindex: n_key_lanes = " + std::to_string(nk) + ": the batch has " + std::to_string(nl) + " lanes");
   s.n_key_lanes = nk; s.n_val_lanes = nl - nk;
   Tuples t(s);
   flat_rows(*a->p, t);
@@ -896,12 +1011,20 @@ int32_t orc_batch_reindex(orc_ctx*, const orc_batch* a, uint32_t nk, orc_batch**
   return DBSP_OK;
 }
 
-int32_t orc_batch_len(const orc_batch* b, u64* n) { *n = b->p->len(); return DBSP_OK; }
-int32_t orc_batch_key_count(orc_ctx*, const orc_batch* b, u64* n) { *n = b->p->nkeys(); return DBSP_OK; }
-int32_t orc_batch_schema(const orc_batch* b, dbsp_schema* out) { *out = b->p->s; return DBSP_OK; }
+int32_t orc_batch_len(const orc_batch* b, u64* n) { NOT_NULL(b, "batch"); NOT_NULL(n, "n_tuples"); *n = b->p->len(); return DBSP_OK; }
+int32_t orc_batch_key_count(orc_ctx* c, const orc_batch* b, u64* n) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(b, "batch");
+  NOT_NULL(n, "n_keys");
+  *n = b->p->nkeys();
+  return DBSP_OK;
+}
+int32_t orc_batch_schema(const orc_batch* b, dbsp_schema* out) { NOT_NULL(b, "batch"); NOT_NULL(out, "out"); *out = b->p->s; return DBSP_OK; }
 
-int32_t orc_batch_download_csr(orc_ctx*, const orc_batch* bb, u64* const* keys, u64* offs, u64* const* vals,
+int32_t orc_batch_download_csr(orc_ctx* c, const orc_batch* bb, u64* const* keys, u64* offs, u64* const* vals,
                                i64* diffs) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(bb, "batch");
   const Batch& b = *bb->p;
   if (keys) for (int l = 0; l < b.K.nl; l++) if (keys[l]) std::copy(b.K.c[l].begin(), b.K.c[l].end(), keys[l]);
   if (offs && b.indexed()) {
@@ -917,22 +1040,32 @@ int32_t orc_batch_device_columns(const orc_batch*, const u64**, const i64**) { r
 struct orc_download;
 int32_t orc_batch_download_begin(orc_ctx*, const orc_batch*, u64* const*, i64*, orc_download**) { return DBSP_ERR_UNSUPPORTED; }
 int32_t orc_download_finish(orc_download*) { return DBSP_OK; }
-int32_t orc_ctx_sync_stats(orc_ctx*, u64* n, double* us, int32_t) { if (n) *n = 0; if (us) *us = 0; return DBSP_OK; }
+int32_t orc_ctx_sync_stats(orc_ctx* c, u64* n, double* us, int32_t) { NOT_NULL(c, "ctx"); if (n) *n = 0; if (us) *us = 0; return DBSP_OK; }
 
 // fast_forward_keys + get_key (operator/time_series/watermark.rs:38-45).
-int32_t orc_batch_last_key(orc_ctx*, const orc_batch* b, u64* key, int32_t* valid) {
+int32_t orc_batch_last_key(orc_ctx* c, const orc_batch* b, u64* key, int32_t* valid) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(b, "batch");
+  NOT_NULL(valid, "valid");
+  CHECK_ARG(key != nullptr || b->p->s.n_key_lanes == 0, "batch_last_key: key is NULL");
   const Batch& B = *b->p;
   *valid = B.K.n > 0;
   if (B.K.n) B.K.get(B.K.n - 1, key);
   return DBSP_OK;
 }
-int32_t orc_batch_clone(const orc_batch* b, orc_batch** out) { *out = wrap(b->p); return DBSP_OK; }
+int32_t orc_batch_clone(const orc_batch* b, orc_batch** out) { NOT_NULL(b, "batch"); NOT_NULL(out, "out"); *out = wrap(b->p); return DBSP_OK; }
 int32_t orc_batch_free(orc_batch* b) { delete b; return DBSP_OK; }
 
 // Builder::push ... done (trace/mod.rs:338-368; ordered/mod.rs:468-479,874-888): the rows are already
 // sorted and consolidated — appended in order, no sort.
-int32_t orc_batch_from_sorted(orc_ctx*, const dbsp_schema* s, const u64* const* cols, const i64* w, u64 n,
+int32_t orc_batch_from_sorted(orc_ctx* c, const dbsp_schema* s, const u64* const* cols, const i64* w, u64 n,
                               int32_t, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_schema(s, WHAT));
+  REFUSE(valid_cols(WHAT, cols, s->n_key_lanes + s->n_val_lanes, n));
+  CHECK_ARG(n == 0 || w != nullptr, "batch_from_sorted: weights is NULL (consolidated rows carry their weights)");
+  ROWS32(n);
   Builder bld(*s);
   const int nk = s->n_key_lanes, nv = s->n_val_lanes;
   u64 key[MAXL], val[MAXL];
@@ -945,13 +1078,51 @@ int32_t orc_batch_from_sorted(orc_ctx*, const dbsp_schema* s, const u64* const* 
   return DBSP_OK;
 }
 
-int32_t orc_spine_new(orc_ctx*, const dbsp_schema* s, orc_spine** out) { *out = new orc_spine(*s); return DBSP_OK; }
-int32_t orc_spine_insert(orc_ctx*, orc_spine* s, const orc_batch* b) { s->s.insert(b->p); return DBSP_OK; }
-int32_t orc_spine_consolidate(orc_ctx*, orc_spine* s, orc_batch** out) { *out = wrap(s->s.consolidate()); return DBSP_OK; }
-int32_t orc_spine_truncate_keys_below(orc_ctx*, orc_spine* s, const u64* key) { s->s.truncate(key); return DBSP_OK; }
-int32_t orc_spine_truncate_values_below(orc_ctx*, orc_spine* s, const u64* val) { s->s.truncate_values(val); return DBSP_OK; }
-int32_t orc_spine_exert(orc_ctx*, orc_spine* s, i64* effort) { s->s.exert(effort); return DBSP_OK; }
+int32_t orc_spine_new(orc_ctx* c, const dbsp_schema* s, orc_spine** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_schema(s, WHAT));
+  *out = new orc_spine(*s);
+  return DBSP_OK;
+}
+int32_t orc_spine_insert(orc_ctx* c, orc_spine* s, const orc_batch* b) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(s, "spine");
+  NOT_NULL(b, "batch");
+  CHECK_ARG(dv::same_schema(s->s.s, b->p->s), "spine_insert: spine and batch differ in schema");
+  s->s.insert(b->p);
+  return DBSP_OK;
+}
+int32_t orc_spine_consolidate(orc_ctx* c, orc_spine* s, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(s, "spine");
+  NOT_NULL(out, "out");
+  *out = wrap(s->s.consolidate());
+  return DBSP_OK;
+}
+int32_t orc_spine_truncate_keys_below(orc_ctx* c, orc_spine* s, const u64* key) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(s, "spine");
+  CHECK_ARG(key != nullptr || s->s.s.n_key_lanes == 0, "spine_truncate_keys_below: key is NULL");
+  s->s.truncate(key);
+  return DBSP_OK;
+}
+int32_t orc_spine_truncate_values_below(orc_ctx* c, orc_spine* s, const u64* val) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(s, "spine");
+  CHECK_ARG(val != nullptr || s->s.s.n_val_lanes == 0, "spine_truncate_values_below: val is NULL");
+  s->s.truncate_values(val);
+  return DBSP_OK;
+}
+int32_t orc_spine_exert(orc_ctx* c, orc_spine* s, i64* effort) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(s, "spine");
+  NOT_NULL(effort, "effort");
+  s->s.exert(effort);
+  return DBSP_OK;
+}
 int32_t orc_spine_len(const orc_spine* s, u64* n, uint32_t* nb) {
+  NOT_NULL(s, "spine");
   if (n) *n = s->s.len();
   if (nb) *nb = (uint32_t)s->s.batches.size();
   return DBSP_OK;
@@ -962,15 +1133,25 @@ int32_t orc_spine_free(orc_spine* s) { delete s; return DBSP_OK; }
 // cursor is a CursorList over the spine's batches and map_times yields each
 // batch's weight separately (:769-776), i.e. delta is joined with every batch
 // and the outputs are consolidated by the Batcher (:845-858).
-int32_t orc_join_delta_trace(orc_ctx*, const orc_batch* delta, const orc_spine* tr, const dbsp_proj* proj,
+int32_t orc_join_delta_trace(orc_ctx* c, const orc_batch* delta, const orc_spine* tr, const dbsp_proj* proj,
                              int32_t delta_is_left, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(delta, "delta");
+  NOT_NULL(tr, "trace");
+  REFUSE(delta_is_left ? valid_join(WHAT, delta->p->s, tr->s.s, proj) : valid_join(WHAT, tr->s.s, delta->p->s, proj));
   Tuples t(proj->out_schema);
   for (auto& b : tr->s.batches) join_into(*delta->p, *b, *proj, !delta_is_left, t);
   *out = wrap(t.build());
   return DBSP_OK;
 }
 
-int32_t orc_join_batches(orc_ctx*, const orc_batch* l, const orc_batch* r, const dbsp_proj* proj, orc_batch** out) {
+int32_t orc_join_batches(orc_ctx* c, const orc_batch* l, const orc_batch* r, const dbsp_proj* proj, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(l, "left");
+  NOT_NULL(r, "right");
+  REFUSE(valid_join(WHAT, l->p->s, r->p->s, proj));
   Tuples t(proj->out_schema);
   join_into(*l->p, *r->p, *proj, false, t);
   *out = wrap(t.build());
@@ -978,7 +1159,13 @@ int32_t orc_join_batches(orc_ctx*, const orc_batch* l, const orc_batch* r, const
 }
 
 // SemiJoinStream::eval (operator/semijoin.rs:100-142).
-int32_t orc_semijoin(orc_ctx*, const orc_batch* pairs, const orc_batch* keys, orc_batch** out) {
+int32_t orc_semijoin(orc_ctx* c, const orc_batch* pairs, const orc_batch* keys, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(pairs, "pairs");
+  NOT_NULL(keys, "keys");
+  CHECK_ARG(dv::same_key_lanes(pairs->p->s, keys->p->s), "semijoin: pairs and keys differ in key lanes (count or type)");
+  CHECK_ARG(keys->p->s.n_val_lanes == 0, "semijoin: keys must be a batch without value lanes");
   const Batch& P = *pairs->p;
   const Batch& Kb = *keys->p;
   // Out: ZSet<Key = (Pairs::Key, Pairs::Val)> (semijoin.rs:47): an OrdZSet over all lanes
@@ -1013,8 +1200,14 @@ int32_t orc_semijoin(orc_ctx*, const orc_batch* pairs, const orc_batch* keys, or
 // 600-684) producing (key, Option<out>) per delta key, then Upsert::eval
 // (operator/upsert.rs:161-208): retract the key's current values in the
 // output trace, insert the new one, consolidate per key.
-int32_t orc_aggregate_delta(orc_ctx*, const orc_batch* delta, const orc_spine* in_tr, const orc_spine* out_tr,
+int32_t orc_aggregate_delta(orc_ctx* c, const orc_batch* delta, const orc_spine* in_tr, const orc_spine* out_tr,
                             int32_t kind, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(delta, "delta");
+  NOT_NULL(in_tr, "in_trace");
+  NOT_NULL(out_tr, "out_trace");
+  REFUSE(dv::valid_aggregate(delta->p->s, in_tr->s.s, out_tr->s.s, kind));
   const Batch& D = *delta->p;
   const dbsp_schema& os = out_tr->s.s;
   int nk = os.n_key_lanes, nov = os.n_val_lanes;
@@ -1079,8 +1272,15 @@ int32_t orc_aggregate_delta(orc_ctx*, const orc_batch* delta, const orc_spine* i
 }
 
 // weigh (operator/aggregate/mod.rs:297-323).
-int32_t orc_weigh(orc_ctx*, const orc_batch* b, const dbsp_expr* f, int32_t mode, orc_batch** out) {
+int32_t orc_weigh(orc_ctx* c, const orc_batch* b, const dbsp_expr* f, int32_t mode, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
   const Batch& B = *b->p;
+  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || mode == DBSP_WEIGH_AVG, "weigh: mode = " + std::to_string(mode) + " is not a weigh mode");
+  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || B.s.n_key_lanes < MAXL, "weigh: WEIGH_AVG adds a key lane and the batch already has 8");
+  CHECK_ARG(mode == DBSP_WEIGH_AVG || B.s.n_key_lanes >= 1, "weigh: WEIGH_LINEAR of a batch without key lanes has no output lanes");
+  REFUSE(dv::valid_expr(f, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, "weigh: f"));
   dbsp_schema s = B.s;
   s.n_val_lanes = 0;
   if (mode == DBSP_WEIGH_AVG) { s.lane_types[s.n_key_lanes] = DBSP_U64; s.n_key_lanes++; }
@@ -1109,7 +1309,12 @@ int32_t orc_weigh(orc_ctx*, const orc_batch* b, const dbsp_expr* f, int32_t mode
 }
 
 // DistinctIncrementalTotal::eval (operator/distinct.rs:196-254).
-int32_t orc_distinct_delta(orc_ctx*, const orc_batch* delta, const orc_spine* integral, orc_batch** out) {
+int32_t orc_distinct_delta(orc_ctx* c, const orc_batch* delta, const orc_spine* integral, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(delta, "delta");
+  NOT_NULL(integral, "delayed_integral");
+  CHECK_ARG(dv::same_schema(delta->p->s, integral->s.s), "distinct_delta: delta and delayed_integral differ in schema");
   const Batch& D = *delta->p;
   Builder bld(D.s);
   std::vector<std::pair<KV, i64>> grp;
@@ -1134,7 +1339,10 @@ int32_t orc_distinct_delta(orc_ctx*, const orc_batch* delta, const orc_spine* in
 }
 
 // IndexedZSet::distinct (algebra/zset/mod.rs:14-38).
-int32_t orc_stream_distinct(orc_ctx*, const orc_batch* b, orc_batch** out) {
+int32_t orc_stream_distinct(orc_ctx* c, const orc_batch* b, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
   const Batch& B = *b->p;
   Builder bld(B.s);
   u64 key[MAXL], val[MAXL];
@@ -1152,8 +1360,15 @@ int32_t orc_stream_distinct(orc_ctx*, const orc_batch* b, orc_batch** out) {
 }
 
 // Window::eval (operator/time_series/window.rs:144-222).
-int32_t orc_window_delta(orc_ctx*, const orc_spine* tr, const orc_batch* delta, int32_t has_prev, const u64* s0,
+int32_t orc_window_delta(orc_ctx* c, const orc_spine* tr, const orc_batch* delta, int32_t has_prev, const u64* s0,
                          const u64* e0, const u64* s1, const u64* e1, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(tr, "trace");
+  NOT_NULL(delta, "delta");
+  CHECK_ARG(dv::same_schema(tr->s.s, delta->p->s), "window_delta: trace and delta differ in schema");
+  CHECK_ARG(s1 && e1, "window_delta: start1 / end1 is NULL");
+  CHECK_ARG(!has_prev || (s0 && e0), "window_delta: start0 / end0 is NULL although has_prev is set");
   const dbsp_schema& s = delta->p->s;
   int nk = s.n_key_lanes;
   Tuples t(s);
@@ -1188,8 +1403,12 @@ int32_t orc_window_delta(orc_ctx*, const orc_spine* tr, const orc_batch* delta, 
 }
 
 // Map/FlatMap::eval + from_tuples (operator/filter_map.rs:563-577,700-724).
-int32_t orc_map_index(orc_ctx*, const orc_batch* b, const dbsp_proj* proj, orc_batch** out) {
+int32_t orc_map_index(orc_ctx* c, const orc_batch* b, const dbsp_proj* proj, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
   const Batch& B = *b->p;
+  REFUSE(dv::valid_proj(proj, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, WHAT));
   Tuples t(proj->out_schema);
   u64 key[MAXL], val[MAXL] = {0}, row[MAXL];
   for (size_t k = 0; k < B.K.n; k++) {
@@ -1216,7 +1435,11 @@ static inline u64 mix64(u64 x) {
   return x ^ (x >> 31);
 }
 // shard_batch (operator/communication/shard.rs:165-199).
-int32_t orc_shard_partition(orc_ctx*, const orc_batch* b, uint32_t P, orc_batch** outs) {
+int32_t orc_shard_partition(orc_ctx* c, const orc_batch* b, uint32_t P, orc_batch** outs) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(b, "batch");
+  NOT_NULL(outs, "outs");
+  CHECK_ARG(P >= 1 && P <= 64, "shard_partition: n_shards = " + std::to_string(P) + ": 1..64 shards");
   const Batch& B = *b->p;
   std::vector<Builder> blds;
   for (uint32_t p = 0; p < P; p++) blds.emplace_back(B.s);
@@ -1257,28 +1480,41 @@ static bool save_flat(FILE* f, const BatchP& b) {
   for (int l = 0; l < nv; l++) if (!wr(f, B.V.c[l].data(), n * 8)) return false;
   return wr(f, B.w.data(), n * 8);
 }
-static bool load_flat(FILE* f, const dbsp_schema& sc, BatchP* out, bool* present_out) {
+// batch `which` (0 = a, 1 = b) of a layer of kind `kind`: checked before anything is allocated for it, and its rows
+// checked — ordered, no duplicate rows, no zero weights — before they become a batch of the trace
+static int32_t load_flat(FILE* f, u64 file_bytes, const dbsp_schema& sc, u64 kind, int which, BatchP* out) {
   u64 present = 0, n = 0;
-  if (!rd(f, &present, 8) || !rd(f, &n, 8)) return false;
-  *present_out = present != 0;
   *out = nullptr;
-  if (!present) return true;
+  if (!rd(f, &present, 8) || !rd(f, &n, 8)) { g_err = "spine_load: truncated file (batch header)"; return DBSP_ERR_INVALID; }
   const int L = sc.n_key_lanes + sc.n_val_lanes;
+  REFUSE(dv::valid_snapshot_batch(kind, which, present, n, L, file_bytes - (u64)ftell(f)));
+  if (!present) return DBSP_OK;
   std::vector<std::vector<u64>> cols((size_t)L, std::vector<u64>(n));
   std::vector<i64> w(n);
-  for (int l = 0; l < L; l++) if (!rd(f, cols[(size_t)l].data(), n * 8)) return false;
-  if (!rd(f, w.data(), n * 8)) return false;
+  for (int l = 0; l < L; l++) if (!rd(f, cols[(size_t)l].data(), n * 8)) { g_err = "spine_load: truncated file (lane)"; return DBSP_ERR_INVALID; }
+  if (!rd(f, w.data(), n * 8)) { g_err = "spine_load: truncated file (weights)"; return DBSP_ERR_INVALID; }
+  u64 inv = 0, dup = 0, zero = 0, prev[MAXL], row[MAXL];
   Builder bld(sc);
-  u64 key[MAXL], val[MAXL];
   for (u64 i = 0; i < n; i++) {
-    for (int l = 0; l < sc.n_key_lanes; l++) key[l] = cols[(size_t)l][i];
-    for (int l = 0; l < sc.n_val_lanes; l++) val[l] = cols[(size_t)(sc.n_key_lanes + l)][i];
-    bld.push(key, val, w[i]);
+    for (int l = 0; l < L; l++) row[l] = cols[(size_t)l][i];
+    if (i) {
+      const int c = cmp_tuples(sc.lane_types, L, prev, row);
+      inv += c > 0;
+      dup += c == 0;
+    }
+    zero += w[i] == 0;
+    bld.push(row, row + sc.n_key_lanes, w[i]);
+    memcpy(prev, row, sizeof(row));
   }
+  CHECK_ARG(!(inv || dup || zero), "spine_load: rows of a batch are not consolidated (" + std::to_string(inv) + " out of order, " +
+                                       std::to_string(dup) + " duplicates, " + std::to_string(zero) + " zero weights)");
   *out = bld.done();
-  return true;
+  return DBSP_OK;
 }
-int32_t orc_spine_save(orc_ctx*, const orc_spine* sp, const char* path) {
+int32_t orc_spine_save(orc_ctx* c, const orc_spine* sp, const char* path) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(sp, "spine");
+  NOT_NULL(path, "path");
   const Spine& s = sp->s;
   FILE* f = fopen(path, "wb");
   if (!f) { g_err = "spine_save: cannot open file"; return DBSP_ERR_INVALID; }
@@ -1296,65 +1532,105 @@ int32_t orc_spine_save(orc_ctx*, const orc_spine* sp, const char* path) {
   if (!ok) { g_err = "spine_save: write failed"; return DBSP_ERR_INVALID; }
   return DBSP_OK;
 }
-int32_t orc_spine_load(orc_ctx*, const char* path, orc_spine** out) {
-  FILE* f = fopen(path, "rb");
-  if (!f) { g_err = "spine_load: cannot open file"; return DBSP_ERR_INVALID; }
+static int32_t load_spine(FILE* f, std::unique_ptr<orc_spine>& sp) {
+  u64 file_bytes = 0;
+  if (fseek(f, 0, SEEK_END) == 0) { file_bytes = (u64)ftell(f); rewind(f); }
   char magic[8];
   dbsp_schema sc;
-  u64 hdr[4];
-  if (!rd(f, magic, 8) || memcmp(magic, SPINE_MAGIC, 8) != 0 || !rd(f, &sc, sizeof(sc)) || !rd(f, hdr, sizeof(hdr))) {
-    fclose(f);
-    g_err = "spine_load: not a spine snapshot";
+  u64 hdr[4], bound[MAXL], vbound[MAXL];
+  if (!rd(f, magic, 8) || memcmp(magic, SPINE_MAGIC, 8) != 0) { g_err = "spine_load: not a spine snapshot (magic)"; return DBSP_ERR_INVALID; }
+  if (!rd(f, &sc, sizeof(sc)) || !rd(f, hdr, sizeof(hdr)) || !rd(f, bound, 8 * MAXL) || !rd(f, vbound, 8 * MAXL)) {
+    g_err = "spine_load: truncated file (header)";
     return DBSP_ERR_INVALID;
   }
-  orc_spine* sp = new orc_spine(sc);
+  REFUSE(dv::valid_snapshot_header(sc, hdr));
+  sp.reset(new orc_spine(sc));
   Spine& s = sp->s;
-  bool ok = rd(f, s.bound, 8 * MAXL) && rd(f, s.vbound, 8 * MAXL) && hdr[3] <= 64;
+  memcpy(s.bound, bound, sizeof(bound));
+  memcpy(s.vbound, vbound, sizeof(vbound));
   s.has_bound = hdr[0] != 0;
   s.has_vbound = hdr[1] != 0;
   s.effort = hdr[2] ? (size_t)hdr[2] : 1;
-  for (u64 i = 0; ok && i < hdr[3]; i++) {
+  for (u64 i = 0; i < hdr[3]; i++) {
     u64 lh[2];
+    if (!rd(f, lh, sizeof(lh))) { g_err = "spine_load: truncated file (layer header)"; return DBSP_ERR_INVALID; }
+    REFUSE(dv::valid_snapshot_kind(lh[0]));
     Spine::Layer l;
-    bool pa = false, pb = false;
-    ok = rd(f, lh, sizeof(lh)) && lh[0] <= (u64)Spine::Layer::COMPLETE && load_flat(f, sc, &l.a, &pa) && load_flat(f, sc, &l.b, &pb);
-    if (!ok) break;
+    int32_t rc = load_flat(f, file_bytes, sc, lh[0], 0, &l.a);
+    if (rc == DBSP_OK) rc = load_flat(f, file_bytes, sc, lh[0], 1, &l.b);
+    if (rc != DBSP_OK) return rc;
+    REFUSE(dv::valid_snapshot_remaining(lh[1], l.a ? l.a->len() : 0, l.b ? l.b->len() : 0));
     l.kind = (Spine::Layer::Kind)lh[0];
-    if (l.kind == Spine::Layer::IN_PROGRESS) {
-      if (!l.a || !l.b) { ok = false; break; }
-      l.m = std::make_shared<Merger>(l.a, l.b);   // the merge restarts; its inputs and its place in the schedule are kept
-    }
+    if (l.kind == Spine::Layer::IN_PROGRESS) l.m = std::make_shared<Merger>(l.a, l.b);   // the merge restarts; its inputs and its place in the schedule are kept
     s.merging.push_back(l);
   }
+  if ((u64)ftell(f) != file_bytes) { g_err = "spine_load: " + std::to_string(file_bytes - (u64)ftell(f)) + " trailing bytes after the last layer"; return DBSP_ERR_INVALID; }
+  return DBSP_OK;
+}
+int32_t orc_spine_load(orc_ctx* c, const char* path, orc_spine** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(path, "path");
+  NOT_NULL(out, "out");
+  FILE* f = fopen(path, "rb");
+  if (!f) { g_err = "spine_load: cannot open file"; return DBSP_ERR_INVALID; }
+  std::unique_ptr<orc_spine> sp;   // a refused file leaves nothing behind
+  const int32_t rc = load_spine(f, sp);
   fclose(f);
-  if (!ok) { delete sp; g_err = "spine_load: truncated or corrupt file"; return DBSP_ERR_INVALID; }
-  s.refresh();
-  *out = sp;
+  if (rc != DBSP_OK) return rc;
+  sp->s.refresh();
+  *out = sp.release();
   return DBSP_OK;
 }
 
 // Communication entry points of the ABI.  The oracle is one worker: identity for world == 1 (shard.rs:111-114);
 // the multi-worker CPU runs use the in-process exchange of oracle/nexmark_workers.cpp / thread_workers.py.
-int32_t orc_comm_create(orc_ctx*, int32_t rank, int32_t world, u64, uint8_t* blob) {
+int32_t orc_comm_create(orc_ctx* c, int32_t rank, int32_t world, u64, uint8_t* blob) {
+  NOT_NULL(c, "ctx");
+  CHECK_ARG(blob != nullptr, "comm_create: blob_out is NULL");
+  CHECK_ARG(world >= 1 && world <= DBSP_COMM_MAX_RANKS, "comm_create: world = " + std::to_string(world) + ": 1..32 ranks");
+  CHECK_ARG(rank >= 0 && rank < world, "comm_create: rank = " + std::to_string(rank) + " is not below world = " + std::to_string(world));
   if (world != 1 || rank != 0) { g_err = "oracle: single worker only"; return DBSP_ERR_UNSUPPORTED; }
   if (blob) memset(blob, 0, DBSP_COMM_BLOB_BYTES);
   return DBSP_OK;
 }
-int32_t orc_comm_connect(orc_ctx*, const uint8_t*) { return DBSP_OK; }
-int32_t orc_comm_destroy(orc_ctx*) { return DBSP_OK; }
-int32_t orc_comm_info(orc_ctx*, int32_t* rank, int32_t* world, u64* bytes) {
+int32_t orc_comm_connect(orc_ctx* c, const uint8_t* blobs) {
+  NOT_NULL(c, "ctx");
+  CHECK_ARG(blobs != nullptr, "comm_connect: blobs is NULL");
+  return DBSP_OK;
+}
+int32_t orc_comm_destroy(orc_ctx* c) { NOT_NULL(c, "ctx"); return DBSP_OK; }
+int32_t orc_comm_info(orc_ctx* c, int32_t* rank, int32_t* world, u64* bytes) {
+  NOT_NULL(c, "ctx");
   if (rank) *rank = 0;
   if (world) *world = 1;
   if (bytes) *bytes = 0;
   return DBSP_OK;
 }
-int32_t orc_shard(orc_ctx*, const orc_batch* b, orc_batch** out) { *out = wrap(b->p); return DBSP_OK; }
-int32_t orc_shard2(orc_ctx*, const orc_batch* a, const orc_batch* b, orc_batch** oa, orc_batch** ob) {
+int32_t orc_shard(orc_ctx* c, const orc_batch* b, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  *out = wrap(b->p);
+  return DBSP_OK;
+}
+int32_t orc_shard2(orc_ctx* c, const orc_batch* a, const orc_batch* b, orc_batch** oa, orc_batch** ob) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(oa, "out_a");
+  NOT_NULL(ob, "out_b");
+  NOT_NULL(a, "a");
+  NOT_NULL(b, "b");
   *oa = wrap(a->p);
   *ob = wrap(b->p);
   return DBSP_OK;
 }
-int32_t orc_gather(orc_ctx*, const orc_batch* b, int32_t, orc_batch** out) { *out = wrap(b->p); return DBSP_OK; }
-int32_t orc_allreduce_max_u64(orc_ctx*, u64*) { return DBSP_OK; }
+int32_t orc_gather(orc_ctx* c, const orc_batch* b, int32_t root, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  CHECK_ARG(root == 0, "gather: root = " + std::to_string(root) + " is not a rank of a group of 1");
+  *out = wrap(b->p);
+  return DBSP_OK;
+}
+int32_t orc_allreduce_max_u64(orc_ctx* c, u64* x) { NOT_NULL(c, "ctx"); NOT_NULL(x, "x"); return DBSP_OK; }
 
 }  // extern "C"

@@ -17,8 +17,8 @@ ORACLE_LIB = os.path.join(ORACLE_DIR, "libdbsp_oracle.so")
 
 
 def build_oracle():
-    src = os.path.join(ORACLE_DIR, "dbsp_oracle.cpp")
-    if not os.path.exists(ORACLE_LIB) or os.path.getmtime(ORACLE_LIB) < os.path.getmtime(src):
+    srcs = [os.path.join(ORACLE_DIR, "dbsp_oracle.cpp"), os.path.join(ROOT, "database-stream-processor_b200", "csrc", "validate.h")]
+    if not os.path.exists(ORACLE_LIB) or os.path.getmtime(ORACLE_LIB) < max(os.path.getmtime(x) for x in srcs):
         subprocess.check_call(["make", "-C", ORACLE_DIR, "-s"])
     return ORACLE_LIB
 
@@ -26,8 +26,9 @@ def build_oracle():
 class OracleBackend(Backend):
     name = "oracle"
 
-    def __init__(self):
-        lib = C.CDLL(build_oracle())
+    def __init__(self, lib_path=None):
+        """lib_path: another build of the oracle (the sanitizer build of oracle/Makefile) instead of the default one."""
+        lib = C.CDLL(lib_path or build_oracle())
         super().__init__(CApi(lib, "orc_"), 0)
 
     def flat(self, b: Batch):

@@ -93,7 +93,9 @@ static int32_t stage_columns(Ctx* ctx, const u64* const* cols, int ncols, const 
 // reference's Merger advances a few thousand rows per call; the GPU merges two whole batches in one launch, so a
 // merge in progress is a fuel account — the two batches stay visible to cursors exactly as long as in the
 // reference (until the fuel paid reaches their length) and the single merge launch happens when the account is
-// settled.  The schedule (which batches meet, when a layer becomes complete) is therefore the reference's.
+// settled.  Which batches meet is the reference's; when a merge completes is not always: the reference's merger
+// spends fuel per value written (fewer than the input rows where rows cancel), this account per input row, so the
+// reference can complete a merge at an earlier insert (DESIGN §2).
 static int32_t merge_bounded(Ctx* ctx, const Batch* x, const Batch* y, const u64* vbound, Batch** out);
 
 static u64 level_len(const SpineLevel& l) {   // MergeState::len (:1034-1041)

@@ -106,9 +106,9 @@ struct Spine {
   std::vector<Batch*> batches;   // cursor view (no references held)
   u64 effort = 1;
   bool has_bound = false;
-  u64 bound[MAXL];
+  u64 bound[MAXL] = {};   // zero until set: dbsp_spine_save writes both arrays whole
   bool has_vbound = false;   // lower_val_bound (spine_fueled.rs:118)
-  u64 vbound[MAXL];
+  u64 vbound[MAXL] = {};
   Ctx* ctx = nullptr;
 };
 

@@ -420,9 +420,9 @@ struct Spine {
   std::vector<BatchP> batches;   // cursor view, largest layer first
   size_t effort = 1;
   bool has_bound = false;
-  u64 bound[MAXL];
+  u64 bound[MAXL] = {};   // zero until set: spine_save writes both arrays whole
   bool has_vbound = false;   // lower_val_bound (spine_fueled.rs:118, 644-656)
-  u64 vbound[MAXL];
+  u64 vbound[MAXL] = {};
   explicit Spine(const dbsp_schema& sc) : s(sc) {}
   const u64* vb() const { return has_vbound ? vbound : nullptr; }
 

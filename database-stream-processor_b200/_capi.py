@@ -12,6 +12,8 @@ import numpy as np
 
 MAX_LANES = 8
 MAX_PREDS = 4
+MAX_INSNS = 64
+MAX_STACK = 16
 
 OK = 0
 ERR_NAMES = {1: "DBSP_ERR_INVALID", 2: "DBSP_ERR_CUDA", 3: "DBSP_ERR_NO_DEVICE", 4: "DBSP_ERR_UNSUPPORTED"}
@@ -22,6 +24,9 @@ OP_COPY, OP_NEG, OP_ADD, OP_SUB, OP_MUL, OP_DIV = range(6)
 CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_IN = range(7)
 AGG_MAX, AGG_MIN, AGG_FOLD_COUNT, AGG_FOLD_SUM, AGG_WCOUNT, AGG_WCOUNT2 = range(6)
 WEIGH_LINEAR, WEIGH_AVG = 0, 1
+(FN_PUSH, FN_NEG, FN_ABS, FN_BNOT, FN_LNOT, FN_ADD, FN_SUB, FN_MUL, FN_DIV, FN_REM, FN_DIVU, FN_REMU, FN_MIN, FN_MAX,
+ FN_MINU, FN_MAXU, FN_AND, FN_OR, FN_XOR, FN_SHL, FN_SHR, FN_SAR, FN_EQ, FN_NE, FN_LT, FN_LE, FN_GT, FN_GE, FN_LTU,
+ FN_LEU, FN_GTU, FN_GEU, FN_IN, FN_SELECT) = range(34)
 
 
 class CSchema(C.Structure):
@@ -50,6 +55,14 @@ class CProj(C.Structure):
     ]
 
 
+class CInsn(C.Structure):
+    _fields_ = [("op", C.c_uint8), ("kind", C.c_uint8), ("idx", C.c_uint8), ("pad_", C.c_uint8 * 5), ("cst", C.c_int64)]
+
+
+class CRowFn(C.Structure):
+    _fields_ = [("out_schema", CSchema), ("n_insn", C.c_uint8), ("pad_", C.c_uint8 * 5), ("code", CInsn * MAX_INSNS)]
+
+
 class DbspError(RuntimeError):
     pass
 
@@ -72,6 +85,8 @@ _SIGS = {
     "batch_from_sorted": [_P, C.POINTER(CSchema), _PP, _P, C.c_uint64, C.c_int32, _PP],
     "upload_begin": [_P, _PP, C.c_uint32, C.c_uint32, _P, C.c_uint64, _PP],
     "batch_from_upload": [_P, _P, C.POINTER(CProj), _PP],
+    "batch_from_table_fn": [_P, _PP, C.c_uint32, _P, C.c_uint64, C.c_int32, C.POINTER(CRowFn), _PP],
+    "batch_from_upload_fn": [_P, _P, C.POINTER(CRowFn), _PP],
     "upload_free": [_P],
     "batch_empty": [_P, C.POINTER(CSchema), _PP],
     "batch_merge": [_P, _P, _P, _PP],
@@ -112,13 +127,17 @@ _SIGS = {
     "spine_load": [_P, C.c_char_p, _PP],
     "join_delta_trace": [_P, _P, _P, C.POINTER(CProj), C.c_int32, _PP],
     "join_batches": [_P, _P, _P, C.POINTER(CProj), _PP],
+    "join_delta_trace_fn": [_P, _P, _P, C.POINTER(CRowFn), C.c_int32, _PP],
+    "join_batches_fn": [_P, _P, _P, C.POINTER(CRowFn), _PP],
     "semijoin": [_P, _P, _P, _PP],
     "aggregate_delta": [_P, _P, _P, _P, C.c_int32, _PP],
     "weigh": [_P, _P, C.POINTER(CExpr), C.c_int32, _PP],
+    "weigh_fn": [_P, _P, C.POINTER(CRowFn), C.c_int32, _PP],
     "distinct_delta": [_P, _P, _P, _PP],
     "stream_distinct": [_P, _P, _PP],
     "window_delta": [_P, _P, _P, C.c_int32, _U64P, _U64P, _U64P, _U64P, _PP],
     "map_index": [_P, _P, C.POINTER(CProj), _PP],
+    "map_index_fn": [_P, _P, C.POINTER(CRowFn), _PP],
     "shard_partition": [_P, _P, C.c_uint32, _PP],
     "comm_create": [_P, C.c_int32, C.c_int32, C.c_uint64, _P],
     "comm_connect": [_P, _P],
@@ -130,6 +149,11 @@ _SIGS = {
     "allreduce_max_u64": [_P, _U64P],
 }
 COMM_BLOB_BYTES = 128
+# The row-function entry points.  The CUDA library exports them all; the CPU oracle of the dbsp_proj tests
+# (oracle/libdbsp_oracle.so) has none, its row-function build (oracle_fn/libdbsp_oracle_fn.so) has them.  A library
+# without them binds every other call, and calling one of them raises DbspError.
+ROWFN_CALLS = {"batch_from_table_fn", "batch_from_upload_fn", "join_delta_trace_fn", "join_batches_fn", "weigh_fn",
+               "map_index_fn"}
 
 
 class CApi:
@@ -139,6 +163,9 @@ class CApi:
         self.lib = lib
         self.prefix = prefix
         for name, argtypes in _SIGS.items():
+            if name in ROWFN_CALLS and not hasattr(lib, prefix + name):
+                setattr(self, "_" + name, self._not_exported(prefix + name))
+                continue
             fn = getattr(lib, prefix + name)  # AttributeError if a symbol is missing
             fn.argtypes = argtypes
             fn.restype = C.c_int32
@@ -152,10 +179,22 @@ class CApi:
         self._proj_table_mask = getattr(lib, prefix + "proj_table_mask")
         self._proj_table_mask.restype = C.c_uint32
         self._proj_table_mask.argtypes = [C.POINTER(CProj)]
+        if hasattr(lib, prefix + "rowfn_table_mask"):
+            self._rowfn_table_mask = getattr(lib, prefix + "rowfn_table_mask")
+            self._rowfn_table_mask.restype = C.c_uint32
+            self._rowfn_table_mask.argtypes = [C.POINTER(CRowFn)]
+        else:
+            self._rowfn_table_mask = self._not_exported(prefix + "rowfn_table_mask")
+
+    @staticmethod
+    def _not_exported(symbol):
+        def refuse(*_):
+            raise DbspError(f"{symbol}: this library has no row functions")
+        return refuse
 
     @staticmethod
     def symbols(prefix: str = "dbsp_"):
-        return [prefix + n for n in list(_SIGS) + ["last_error", "ctx_stream", "proj_table_mask"]]
+        return [prefix + n for n in list(_SIGS) + ["last_error", "ctx_stream", "proj_table_mask", "rowfn_table_mask"]]
 
     def check(self, rc: int, what: str):
         if rc != OK:

@@ -519,6 +519,22 @@ int32_t dbsp_batch_from_table(dbsp_ctx* ctx, const uint64_t* const* cols, uint32
   *out = H(b);
   return DBSP_OK;
 }
+int32_t dbsp_batch_from_table_fn(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n_cols, const int64_t* w,
+                                 uint64_t n, int32_t on_device, const dbsp_rowfn* fn, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "batch_from_table_fn: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
+  REFUSE(dv::valid_rowfn(fn, (int)n_cols, (int)n_cols, (int)n_cols, WHAT));
+  REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, dv::rowfn_table_mask(*fn)));
+  ROWS32(n);
+  BufP hold;
+  Cols dc;
+  const i64* dw;
+  TRY(stage_columns(ctx, cols, (int)n_cols, w, n, on_device, &hold, &dc, &dw, rowfn_used_mask(*fn, 0)));
+  Batch* b = nullptr;
+  TRY(project_and_consolidate(ctx, dc, 0, (int)n_cols, dw, n, *fn, &b));
+  *out = H(b);
+  return DBSP_OK;
+}
 
 struct dbsp_upload {
   Ctx* ctx;
@@ -534,6 +550,10 @@ struct dbsp_upload {
 uint32_t dbsp_proj_table_mask(const dbsp_proj* proj) {
   if (!dv::valid_proj(proj, MAXL, MAXL, MAXL, "proj_table_mask").empty()) return 0;
   return dv::proj_table_mask(*proj);
+}
+uint32_t dbsp_rowfn_table_mask(const dbsp_rowfn* fn) {
+  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "rowfn_table_mask").empty()) return 0;
+  return dv::rowfn_table_mask(*fn);
 }
 
 int32_t dbsp_upload_begin(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n_cols, uint32_t col_mask,
@@ -603,6 +623,21 @@ int32_t dbsp_batch_from_upload(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_proj* p
   CUDA_TRY(cudaStreamWaitEvent(ctx->stream, u->done, 0));   // compute stream waits for the copy
   Batch* b = nullptr;
   TRY(project_and_consolidate(ctx, u->dc, 0, u->n_cols, u->dw, u->n, *proj, &b));
+  *out = H(b);
+  return DBSP_OK;
+}
+int32_t dbsp_batch_from_upload_fn(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_rowfn* fn, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(u, "upload");
+  CHECK_ARG(u->ctx == ctx, "batch_from_upload_fn: upload belongs to another context");
+  REFUSE(dv::valid_rowfn(fn, u->n_cols, u->n_cols, u->n_cols, WHAT));
+  {
+    const unsigned missing = dv::rowfn_table_mask(*fn) & ~u->col_mask;
+    CHECK_ARG(missing == 0, "batch_from_upload_fn: fn reads column " + std::to_string(__builtin_ctz(missing | 0x100u)) + ", which col_mask left out of the upload");
+  }
+  CUDA_TRY(cudaStreamWaitEvent(ctx->stream, u->done, 0));   // compute stream waits for the copy
+  Batch* b = nullptr;
+  TRY(project_and_consolidate(ctx, u->dc, 0, u->n_cols, u->dw, u->n, *fn, &b));
   *out = H(b);
   return DBSP_OK;
 }
@@ -1252,6 +1287,10 @@ static std::string valid_join(const char* what, const dbsp_schema& left, const d
   if (!dv::same_key_lanes(left, right)) return std::string(what) + ": the two inputs differ in key lanes (count or type)";
   return dv::valid_proj(p, left.n_key_lanes, left.n_val_lanes, right.n_val_lanes, what);
 }
+static std::string valid_join_fn(const char* what, const dbsp_schema& left, const dbsp_schema& right, const dbsp_rowfn* f) {
+  if (!dv::same_key_lanes(left, right)) return std::string(what) + ": the two inputs differ in key lanes (count or type)";
+  return dv::valid_rowfn(f, left.n_key_lanes, left.n_val_lanes, right.n_val_lanes, what);
+}
 
 int32_t dbsp_join_delta_trace(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* t, const dbsp_proj* p, int32_t dl,
                               dbsp_batch** out) { ENTER(ctx);
@@ -1266,6 +1305,19 @@ int32_t dbsp_join_batches(dbsp_ctx* ctx, const dbsp_batch* l, const dbsp_batch* 
   NOT_NULL(r, "right");
   REFUSE(valid_join(WHAT, B(l)->s, B(r)->s, p));
   OUT1(op_join_batches(ctx, B(l), B(r), p, &o__)) }
+int32_t dbsp_join_delta_trace_fn(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* t, const dbsp_rowfn* f, int32_t dl,
+                                 dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(d, "delta");
+  NOT_NULL(t, "trace");
+  REFUSE(dl ? valid_join_fn(WHAT, B(d)->s, t->s, f) : valid_join_fn(WHAT, t->s, B(d)->s, f));
+  OUT1(op_join_delta_trace(ctx, B(d), t, f, dl, &o__)) }
+int32_t dbsp_join_batches_fn(dbsp_ctx* ctx, const dbsp_batch* l, const dbsp_batch* r, const dbsp_rowfn* f, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(l, "left");
+  NOT_NULL(r, "right");
+  REFUSE(valid_join_fn(WHAT, B(l)->s, B(r)->s, f));
+  OUT1(op_join_batches(ctx, B(l), B(r), f, &o__)) }
 int32_t dbsp_semijoin(dbsp_ctx* ctx, const dbsp_batch* pairs, const dbsp_batch* keys, dbsp_batch** out) { ENTER(ctx);
   NOT_NULL(out, "out");
   NOT_NULL(pairs, "pairs");
@@ -1288,6 +1340,15 @@ int32_t dbsp_weigh(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_expr* f, int32
   CHECK_ARG(mode == DBSP_WEIGH_LINEAR || B(b)->s.n_key_lanes < MAXL, "weigh: WEIGH_AVG adds a key lane and the batch already has 8");
   CHECK_ARG(mode == DBSP_WEIGH_AVG || B(b)->s.n_key_lanes >= 1, "weigh: WEIGH_LINEAR of a batch without key lanes has no output lanes");
   REFUSE(dv::valid_expr(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, "weigh: f"));
+  OUT1(op_weigh(ctx, B(b), f, mode, &o__)) }
+int32_t dbsp_weigh_fn(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_rowfn* f, int32_t mode, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || mode == DBSP_WEIGH_AVG, "weigh_fn: mode = " + std::to_string(mode) + " is not a weigh mode");
+  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || B(b)->s.n_key_lanes < MAXL, "weigh_fn: WEIGH_AVG adds a key lane and the batch already has 8");
+  CHECK_ARG(mode == DBSP_WEIGH_AVG || B(b)->s.n_key_lanes >= 1, "weigh_fn: WEIGH_LINEAR of a batch without key lanes has no output lanes");
+  REFUSE(dv::valid_rowfn(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT));
+  CHECK_ARG(f->out_schema.n_key_lanes + f->out_schema.n_val_lanes == 1, "weigh_fn: fn.out_schema must have one lane (the factor)");
   OUT1(op_weigh(ctx, B(b), f, mode, &o__)) }
 int32_t dbsp_distinct_delta(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* i, dbsp_batch** out) { ENTER(ctx);
   NOT_NULL(out, "out");
@@ -1314,6 +1375,11 @@ int32_t dbsp_map_index(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_proj* p, d
   NOT_NULL(b, "batch");
   REFUSE(dv::valid_proj(p, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT));
   OUT1(op_map_index(ctx, B(b), p, &o__)) }
+int32_t dbsp_map_index_fn(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_rowfn* f, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  REFUSE(dv::valid_rowfn(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT));
+  OUT1(op_map_index(ctx, B(b), f, &o__)) }
 int32_t dbsp_shard_partition(dbsp_ctx* ctx, const dbsp_batch* b, uint32_t P, dbsp_batch** outs) { ENTER(ctx);
   NOT_NULL(b, "batch");
   NOT_NULL(outs, "outs");

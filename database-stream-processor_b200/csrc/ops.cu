@@ -89,6 +89,125 @@ __device__ __forceinline__ bool project(const dbsp_proj& p, const Env& e, u64* r
   return ok;
 }
 
+// Row function (dbsp_rowfn): the postfix program leaves the output lanes and the keep flag in st[0..L].  The program
+// is a kernel parameter, the same for every thread, so the dispatch is warp-uniform; the stack is a local array
+// indexed by the (uniform) depth.  validate.h has checked the depths and sources, and every operation is total.
+template <class E>
+__device__ __forceinline__ void run_rowfn(const dbsp_rowfn& f, const E& e, u64* st) {
+  int sp = 0;
+#pragma unroll 1
+  for (int pc = 0; pc < f.n_insn; pc++) {
+    const dbsp_insn& in = f.code[pc];
+    const int op = in.op;
+    if (op == DBSP_FN_PUSH) {
+      u64 v;
+      switch (in.kind) {
+        case DBSP_SRC_KEY: v = e.k(in.idx); break;
+        case DBSP_SRC_LVAL: v = e.l(in.idx); break;
+        case DBSP_SRC_RVAL: v = e.r(in.idx); break;
+        default: v = (u64)in.cst;
+      }
+      st[sp++] = v;
+      continue;
+    }
+    if (op <= DBSP_FN_LNOT) {
+      const u64 a = st[sp - 1];
+      u64 r;
+      switch (op) {
+        case DBSP_FN_NEG: r = (u64)0 - a; break;
+        case DBSP_FN_ABS: r = (i64)a < 0 ? (u64)0 - a : a; break;
+        case DBSP_FN_BNOT: r = ~a; break;
+        default: r = a == 0;
+      }
+      st[sp - 1] = r;
+      continue;
+    }
+    if (op == DBSP_FN_SELECT) {
+      st[sp - 3] = st[sp - 3] ? st[sp - 2] : st[sp - 1];
+      sp -= 2;
+      continue;
+    }
+    const u64 b = st[--sp], a = st[sp - 1];
+    const i64 sa = (i64)a, sb = (i64)b;
+    u64 r;
+    switch (op) {
+      case DBSP_FN_ADD: r = a + b; break;
+      case DBSP_FN_SUB: r = a - b; break;
+      case DBSP_FN_MUL: r = a * b; break;
+      case DBSP_FN_DIV: r = sb == 0 ? 0 : sb == -1 ? (u64)0 - a : (u64)(sa / sb); break;   // no MIN / -1 trap
+      case DBSP_FN_REM: r = (sb == 0 || sb == -1) ? 0 : (u64)(sa % sb); break;
+      case DBSP_FN_DIVU: r = b == 0 ? 0 : a / b; break;
+      case DBSP_FN_REMU: r = b == 0 ? 0 : a % b; break;
+      case DBSP_FN_MIN: r = sa < sb ? a : b; break;
+      case DBSP_FN_MAX: r = sa > sb ? a : b; break;
+      case DBSP_FN_MINU: r = a < b ? a : b; break;
+      case DBSP_FN_MAXU: r = a > b ? a : b; break;
+      case DBSP_FN_AND: r = a & b; break;
+      case DBSP_FN_OR: r = a | b; break;
+      case DBSP_FN_XOR: r = a ^ b; break;
+      case DBSP_FN_SHL: r = a << (b & 63); break;
+      case DBSP_FN_SHR: r = a >> (b & 63); break;
+      case DBSP_FN_SAR: r = (u64)(sa >> (b & 63)); break;
+      case DBSP_FN_EQ: r = a == b; break;
+      case DBSP_FN_NE: r = a != b; break;
+      case DBSP_FN_LT: r = sa < sb; break;
+      case DBSP_FN_LE: r = sa <= sb; break;
+      case DBSP_FN_GT: r = sa > sb; break;
+      case DBSP_FN_GE: r = sa >= sb; break;
+      case DBSP_FN_LTU: r = a < b; break;
+      case DBSP_FN_LEU: r = a <= b; break;
+      case DBSP_FN_GTU: r = a > b; break;
+      case DBSP_FN_GEU: r = a >= b; break;
+      default: r = a < 64 && ((b >> a) & 1);   // DBSP_FN_IN
+    }
+    st[sp - 1] = r;
+  }
+}
+
+// The closure forms the kernels that evaluate closures are instantiated on (dbsp_proj / dbsp_rowfn; for weigh
+// dbsp_expr / dbsp_rowfn).  fn_keep: the row passes the filter; fn_emit: put(l, output lane l) for l < nl;
+// project: both, into row[]; fn_factor: the weigh factor (0 for a filtered row) and whether the row counts.
+template <class E>
+__device__ __forceinline__ bool fn_keep(const dbsp_proj& p, const E& e) {
+  bool ok = true;
+  for (int q = 0; q < p.n_pred; q++) ok = ok && pred_ok(p.pred[q], e);
+  return ok;
+}
+template <class E, class Put>
+__device__ __forceinline__ void fn_emit(const dbsp_proj& p, const E& e, int nl, Put put) {
+  for (int l = 0; l < nl; l++) put(l, expr_val(p.out[l], e));
+}
+template <class E>
+__device__ __forceinline__ bool fn_keep(const dbsp_rowfn& f, const E& e) {
+  u64 st[DBSP_MAX_STACK];
+  run_rowfn(f, e, st);
+  return st[f.out_schema.n_key_lanes + f.out_schema.n_val_lanes] != 0;
+}
+template <class E, class Put>
+__device__ __forceinline__ void fn_emit(const dbsp_rowfn& f, const E& e, int nl, Put put) {
+  u64 st[DBSP_MAX_STACK];
+  run_rowfn(f, e, st);
+  for (int l = 0; l < nl; l++) put(l, st[l]);
+}
+__device__ __forceinline__ bool project(const dbsp_rowfn& f, const Env& e, u64* row) {
+  u64 st[DBSP_MAX_STACK];
+  run_rowfn(f, e, st);
+  const int nl = f.out_schema.n_key_lanes + f.out_schema.n_val_lanes;
+  for (int l = 0; l < nl; l++) row[l] = st[l];
+  return st[nl] != 0;
+}
+__device__ __forceinline__ bool fn_factor(const dbsp_expr& fx, const Env& e, u64* fv) {
+  *fv = expr_val(fx, e);
+  return true;
+}
+__device__ __forceinline__ bool fn_factor(const dbsp_rowfn& f, const Env& e, u64* fv) {
+  u64 st[DBSP_MAX_STACK];
+  run_rowfn(f, e, st);
+  const bool keep = st[1] != 0;   // one output lane
+  *fv = keep ? st[0] : 0;
+  return keep;
+}
+
 // flat_map_index over a raw table (filter_map.rs:700-724) / map_index over a
 // batch, in one pass and order preserving: a CTA evaluates the predicates of its PROJ_ROWS rows, a decoupled
 // look-back over the CTA totals gives it its output base, and the survivors' output rows are evaluated and written
@@ -97,8 +216,9 @@ __device__ __forceinline__ bool project(const dbsp_proj& p, const Env& e, u64* r
 // (*d_m): the census of consolidate_rows returns it.  identity != 0 (no predicates): output slot = input row.
 constexpr int PROJ_IT = 4;
 constexpr int PROJ_ROWS = TB * PROJ_IT;
+template <class F>
 __global__ void __launch_bounds__(TB)
-k_project_rows(Cols in, int nk_in, const i64* w, u64 n, dbsp_proj proj, int identity, u32 ntiles, u32* ticket,
+k_project_rows(Cols in, int nk_in, const i64* w, u64 n, F proj, int identity, u32 ntiles, u32* ticket,
                u64* status, MCols out, i64* out_w, u32* d_m) {
   static_assert(PROJ_IT * (TB / 32) == 32, "one warp scans the per-(round, warp) counts");
   __shared__ u32 s_tile;
@@ -112,7 +232,7 @@ k_project_rows(Cols in, int nk_in, const i64* w, u64 n, dbsp_proj proj, int iden
       const u64 i = base + (u64)it * TB + tid;
       if (i < n) {
         const ColEnv e{in, nk_in, i};
-        for (int l = 0; l < nl; l++) out.c[l][i] = expr_val(proj.out[l], e);
+        fn_emit(proj, e, nl, [&](int l, u64 v) { out.c[l][i] = v; });
         out_w[i] = w ? w[i] : 1;
       }
     }
@@ -128,8 +248,7 @@ k_project_rows(Cols in, int nk_in, const i64* w, u64 n, dbsp_proj proj, int iden
     bool ok = false;
     if (i < n) {
       const ColEnv e{in, nk_in, i};
-      ok = true;
-      for (int q = 0; q < proj.n_pred; q++) ok = ok && pred_ok(proj.pred[q], e);
+      ok = fn_keep(proj, e);
     }
     const unsigned m = __ballot_sync(0xffffffffu, ok);
     if (lane == 0) s_cnt[it * (TB / 32) + wid] = __popc(m);
@@ -162,7 +281,7 @@ k_project_rows(Cols in, int nk_in, const i64* w, u64 n, dbsp_proj proj, int iden
     const u64 i = base_row + (u64)it * TB + tid;
     const u64 pos = base + s_off[it * (TB / 32) + wid] + ((rk >> (8 * it)) & 0xffu);
     const ColEnv e{in, nk_in, i};
-    for (int l = 0; l < nl; l++) out.c[l][pos] = expr_val(proj.out[l], e);
+    fn_emit(proj, e, nl, [&](int l, u64 v) { out.c[l][pos] = v; });
     out_w[pos] = w ? w[i] : 1;
   }
 }
@@ -331,9 +450,10 @@ k_row_counts_scan(const u32* __restrict__ ki, const u32* __restrict__ ktot, u64 
 // bisection per 1024 slots instead of one per slot.  Consecutive slots read consecutive trace rows and
 // the same / adjacent delta rows, and write consecutive output rows.
 constexpr int PF_TILE = 1024, PF_SMEM_ROWS = 3072;
+template <class F>
 __global__ void __launch_bounds__(256)
 k_probe_fill(Cols D, const i64* wD, u64 nd, BatchRefs tr, int nk, int nvD, int nvT, const u32* lo, const u32* cnt,
-             const u32* ki, const u32* exscan, u64 total, int proj_mode, int delta_is_left, dbsp_proj proj, MCols out,
+             const u32* ki, const u32* exscan, u64 total, int proj_mode, int delta_is_left, F proj, MCols out,
              i64* out_w) {
   __shared__ u32 s_ex[PF_SMEM_ROWS + 1];
   __shared__ u64 s_rows[2];
@@ -634,19 +754,21 @@ __global__ void k_agg_extremum(Cols K, u64 nkeys, int nk, int nv, BatchRefs tr, 
 
 // weigh (aggregate/mod.rs:297-323): per row f(k,v)*w; AVG mode emits the
 // (sum, count) pair weight as two rows (K,0) / (K,1).
-__global__ void k_weigh(Cols B, const i64* w, u64 n, int nk, int nv, dbsp_expr fx, int mode, MCols out, i64* out_w) {
+template <class F>
+__global__ void k_weigh(Cols B, const i64* w, u64 n, int nk, int nv, F fx, int mode, MCols out, i64* out_w) {
   u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   u64 lanes[MAXL];
   for (int l = 0; l < nk + nv; l++) lanes[l] = B.c[l][i];
   Env e{lanes, lanes + nk, lanes + nk};
-  u64 fv = expr_val(fx, e);
+  u64 fv;
+  const bool counted = fn_factor(fx, e, &fv);
   if (mode == DBSP_WEIGH_AVG) {
     for (int l = 0; l < nk; l++) { out.c[l][2 * i] = lanes[l]; out.c[l][2 * i + 1] = lanes[l]; }
     out.c[nk][2 * i] = 0;
     out.c[nk][2 * i + 1] = 1;
     out_w[2 * i] = (i64)(fv * (u64)w[i]);
-    out_w[2 * i + 1] = w[i];
+    out_w[2 * i + 1] = counted ? w[i] : 0;
   } else {
     for (int l = 0; l < nk; l++) out.c[l][i] = lanes[l];
     out_w[i] = (i64)(fv * (u64)w[i]);
@@ -856,20 +978,40 @@ unsigned proj_used_mask(const dbsp_proj& p, int nk_in) {
   for (int i = 0; i < p.n_pred; i++) { use(p.pred[i].a); use(p.pred[i].b); }
   return mask;
 }
-static int used_lanes(const dbsp_proj& p, int n_in_lanes, int nk_in = 0) {
-  int c = __builtin_popcount(proj_used_mask(p, nk_in) & ((1u << n_in_lanes) - 1));
+unsigned rowfn_used_mask(const dbsp_rowfn& f, int nk_in) {
+  unsigned mask = 0;
+  for (int i = 0; i < f.n_insn; i++) {
+    const dbsp_insn& in = f.code[i];
+    if (in.op != DBSP_FN_PUSH) continue;
+    if (in.kind == DBSP_SRC_KEY) mask |= 1u << in.idx;
+    else if (in.kind == DBSP_SRC_LVAL || in.kind == DBSP_SRC_RVAL) mask |= 1u << (nk_in + in.idx);
+  }
+  return mask;
+}
+static unsigned used_mask(const dbsp_proj& p, int nk_in) { return proj_used_mask(p, nk_in); }
+static unsigned used_mask(const dbsp_rowfn& f, int nk_in) { return rowfn_used_mask(f, nk_in); }
+template <class F>
+static int used_lanes(const F& p, int n_in_lanes, int nk_in = 0) {
+  int c = __builtin_popcount(used_mask(p, nk_in) & ((1u << n_in_lanes) - 1));
   return c;
+}
+// whether the closure can drop a row: predicates, or a keep flag that is not a non-zero constant
+static bool filters(const dbsp_proj& p) { return p.n_pred > 0; }
+static bool filters(const dbsp_rowfn& f) {
+  const dbsp_insn& last = f.code[f.n_insn - 1];   // validated: at least the keep flag is pushed
+  return !(last.op == DBSP_FN_PUSH && last.kind == DBSP_SRC_CONST && last.cst != 0);
 }
 
 // project rows of (in cols) through proj, then consolidate.
+template <class F>
 int32_t project_and_consolidate(Ctx* ctx, const Cols& in, int nk_in, int n_in_lanes, const i64* w, u64 n,
-                                const dbsp_proj& proj, Batch** out) {
+                                const F& proj, Batch** out) {
   const dbsp_schema& os = proj.out_schema;
   int Lo = os.n_key_lanes + os.n_val_lanes;
   if (n == 0) { *out = batch_new_empty(ctx, os); return DBSP_OK; }
   ROWS32(n, "map_index / flat_map_index");
   const unsigned g = (unsigned)((n + PROJ_ROWS - 1) / PROJ_ROWS);
-  const bool filtered = proj.n_pred > 0;
+  const bool filtered = filters(proj);
   const u64 m = n;   // upper bound when a filter is present
   u64* status = nullptr;
   u32* ticket = nullptr;
@@ -894,6 +1036,8 @@ int32_t project_and_consolidate(Ctx* ctx, const Cols& in, int nk_in, int n_in_la
   LAUNCH_COUNT(ctx);
   return consolidate_rows(ctx, os, t.cc(), t.w, m, &t.buf, out, d_m);
 }
+template int32_t project_and_consolidate(Ctx*, const Cols&, int, int, const i64*, u64, const dbsp_proj&, Batch**);
+template int32_t project_and_consolidate(Ctx*, const Cols&, int, int, const i64*, u64, const dbsp_rowfn&, Batch**);
 
 // Probe `delta` against every batch of `trace` and expand the matches.
 // proj == nullptr: gather the matching trace rows unchanged.
@@ -924,7 +1068,8 @@ static int32_t key_segments(Ctx* ctx, const Batch* b, int nk, BufP* kstart, BufP
 
 // Probe `delta` against (up to MAX_REFS) batches of `trace` and expand the matches.
 // proj == nullptr: gather the matching trace rows unchanged.
-static int32_t probe_chunk(Ctx* ctx, const Batch* delta, int nk, Batch* const* tb, int nb, const dbsp_proj* proj,
+template <class F>
+static int32_t probe_chunk(Ctx* ctx, const Batch* delta, int nk, Batch* const* tb, int nb, const F* proj,
                            int delta_is_left, const dbsp_schema& out_schema, const u64* kstart, const u32* ki,
                            const u32* d_nkeys, Batch** out) {
   cudaStream_t st = ctx->stream;
@@ -978,7 +1123,7 @@ static int32_t probe_chunk(Ctx* ctx, const Batch* delta, int nk, Batch* const* t
   }
   if (total == 0) { *out = batch_new_empty(ctx, out_schema); return DBSP_OK; }
   int Lo = out_schema.n_key_lanes + out_schema.n_val_lanes;
-  dbsp_proj pj;
+  F pj;
   if (proj) pj = *proj; else memset(&pj, 0, sizeof(pj));
   TmpRows t;
   TRY(tmp_alloc(ctx, Lo, total, &t));
@@ -996,7 +1141,8 @@ static int32_t probe_chunk(Ctx* ctx, const Batch* delta, int nk, Batch* const* t
 
 static int32_t merge_tree(Ctx* ctx, std::vector<Batch*>& parts, const dbsp_schema& s, Batch** out);
 
-static int32_t probe_spine(Ctx* ctx, const Batch* delta, int nk, const Spine* trace, const dbsp_proj* proj,
+template <class F>
+static int32_t probe_spine(Ctx* ctx, const Batch* delta, int nk, const Spine* trace, const F* proj,
                            int delta_is_left, const dbsp_schema& out_schema, Batch** out) {
   const size_t nb = trace->batches.size();
   if (delta->n == 0 || nb == 0) { *out = batch_new_empty(ctx, out_schema); return DBSP_OK; }
@@ -1016,20 +1162,26 @@ static int32_t probe_spine(Ctx* ctx, const Batch* delta, int nk, const Spine* tr
 }
 
 // JoinTrace::eval (operator/join.rs:732-863)
-int32_t op_join_delta_trace(Ctx* ctx, const Batch* delta, const Spine* trace, const dbsp_proj* proj, int delta_is_left,
+template <class F>
+int32_t op_join_delta_trace(Ctx* ctx, const Batch* delta, const Spine* trace, const F* proj, int delta_is_left,
                             Batch** out) {
   if (delta->s.n_key_lanes != trace->s.n_key_lanes) { set_error("join: key lanes differ"); return DBSP_ERR_INVALID; }
   return probe_spine(ctx, delta, delta->s.n_key_lanes, trace, proj, delta_is_left, proj->out_schema, out);
 }
 
 // Join::eval (operator/join.rs:436-473)
-int32_t op_join_batches(Ctx* ctx, const Batch* l, const Batch* r, const dbsp_proj* proj, Batch** out) {
+template <class F>
+int32_t op_join_batches(Ctx* ctx, const Batch* l, const Batch* r, const F* proj, Batch** out) {
   Spine sp;
   sp.s = r->s;
   sp.ctx = ctx;
   if (r->n) sp.batches.push_back((Batch*)r);
   return op_join_delta_trace(ctx, l, &sp, proj, 1, out);
 }
+template int32_t op_join_delta_trace(Ctx*, const Batch*, const Spine*, const dbsp_proj*, int, Batch**);
+template int32_t op_join_delta_trace(Ctx*, const Batch*, const Spine*, const dbsp_rowfn*, int, Batch**);
+template int32_t op_join_batches(Ctx*, const Batch*, const Batch*, const dbsp_proj*, Batch**);
+template int32_t op_join_batches(Ctx*, const Batch*, const Batch*, const dbsp_rowfn*, Batch**);
 
 // distinct keys (first nk lanes) of a batch as an OrdZSet<K> batch with weight 1
 static int32_t distinct_keys(Ctx* ctx, const Batch* b, int nk, Batch** out) {
@@ -1101,7 +1253,7 @@ int32_t op_aggregate_delta(Ctx* ctx, const Batch* delta, const Spine* in_tr, con
   // 2b. general path: the keys' value groups, weights summed over batches
   Batch* G = nullptr;
   if (!N) {
-    rc = probe_spine(ctx, keys, nk, in_tr, nullptr, 1, in_tr->s, &G);
+    rc = probe_spine(ctx, keys, nk, in_tr, (const dbsp_proj*)nullptr, 1, in_tr->s, &G);
     if (rc) { batch_unref(keys); return rc; }
   }
   // 3. aggregate per key -> rows (key, new value) with weight +1
@@ -1140,7 +1292,7 @@ int32_t op_aggregate_delta(Ctx* ctx, const Batch* delta, const Spine* in_tr, con
   if (G) batch_unref(G);
   // 4. current values of those keys in the output trace, negated
   Batch* O = nullptr;
-  rc = probe_spine(ctx, keys, nk, out_tr, nullptr, 1, os, &O);
+  rc = probe_spine(ctx, keys, nk, out_tr, (const dbsp_proj*)nullptr, 1, os, &O);
   batch_unref(keys);
   if (rc) { batch_unref(N); return rc; }
   // 5. consolidate(+new, -old) per key == merge of two consolidated batches
@@ -1173,7 +1325,8 @@ int32_t op_neg(Ctx* ctx, const Batch* a, Batch** out) {
 }
 
 // weigh (operator/aggregate/mod.rs:297-323)
-int32_t op_weigh(Ctx* ctx, const Batch* b, const dbsp_expr* f, int mode, Batch** out) {
+template <class F>
+int32_t op_weigh(Ctx* ctx, const Batch* b, const F* f, int mode, Batch** out) {
   int nk = b->s.n_key_lanes, nv = b->s.n_val_lanes;
   dbsp_schema os;
   memset(&os, 0, sizeof(os));
@@ -1188,6 +1341,8 @@ int32_t op_weigh(Ctx* ctx, const Batch* b, const dbsp_expr* f, int mode, Batch**
   LAUNCH_COUNT(ctx);
   return consolidate_rows(ctx, os, t.cc(), t.w, m, &t.buf, out);
 }
+template int32_t op_weigh(Ctx*, const Batch*, const dbsp_expr*, int, Batch**);
+template int32_t op_weigh(Ctx*, const Batch*, const dbsp_rowfn*, int, Batch**);
 
 // DistinctIncrementalTotal::eval (operator/distinct.rs:196-254)
 int32_t op_distinct_delta(Ctx* ctx, const Batch* delta, const Spine* integral, Batch** out) {
@@ -1336,9 +1491,12 @@ int32_t op_window_delta(Ctx* ctx, const Spine* trace, const Batch* delta, int ha
 }
 
 // Map/FlatMap/Index::eval + from_tuples (operator/filter_map.rs:563-577,700-724)
-int32_t op_map_index(Ctx* ctx, const Batch* b, const dbsp_proj* proj, Batch** out) {
+template <class F>
+int32_t op_map_index(Ctx* ctx, const Batch* b, const F* proj, Batch** out) {
   return project_and_consolidate(ctx, b->cols(), b->s.n_key_lanes, b->nl(), b->w, b->n, *proj, out);
 }
+template int32_t op_map_index(Ctx*, const Batch*, const dbsp_proj*, Batch**);
+template int32_t op_map_index(Ctx*, const Batch*, const dbsp_rowfn*, Batch**);
 
 // shard_batch (operator/communication/shard.rs:165-199)
 int32_t op_shard_partition(Ctx* ctx, const Batch* b, u32 P, Batch** outs) {

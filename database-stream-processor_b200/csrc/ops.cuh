@@ -7,20 +7,27 @@
 
 int32_t compact_ordered(Ctx* ctx, const dbsp_schema& s, const Cols& in, const i64* w, const u32* keep, u64 n, Batch** out);
 unsigned proj_used_mask(const dbsp_proj& p, int nk_in);
+unsigned rowfn_used_mask(const dbsp_rowfn& f, int nk_in);
+// The closure-taking operators, for F = dbsp_proj and F = dbsp_rowfn (weigh: dbsp_expr and dbsp_rowfn).
+template <class F>
 int32_t project_and_consolidate(Ctx* ctx, const Cols& in, int nk_in, int n_in_lanes, const i64* w, u64 n,
-                                const dbsp_proj& proj, Batch** out);
-int32_t op_join_delta_trace(Ctx* ctx, const Batch* delta, const Spine* trace, const dbsp_proj* proj, int delta_is_left,
+                                const F& proj, Batch** out);
+template <class F>
+int32_t op_join_delta_trace(Ctx* ctx, const Batch* delta, const Spine* trace, const F* proj, int delta_is_left,
                             Batch** out);
-int32_t op_join_batches(Ctx* ctx, const Batch* l, const Batch* r, const dbsp_proj* proj, Batch** out);
+template <class F>
+int32_t op_join_batches(Ctx* ctx, const Batch* l, const Batch* r, const F* proj, Batch** out);
 int32_t op_aggregate_delta(Ctx* ctx, const Batch* delta, const Spine* in_tr, const Spine* out_tr, int kind, Batch** out);
 int32_t op_neg(Ctx* ctx, const Batch* a, Batch** out);
-int32_t op_weigh(Ctx* ctx, const Batch* b, const dbsp_expr* f, int mode, Batch** out);
+template <class F>
+int32_t op_weigh(Ctx* ctx, const Batch* b, const F* f, int mode, Batch** out);
 int32_t op_distinct_delta(Ctx* ctx, const Batch* delta, const Spine* integral, Batch** out);
 int32_t op_stream_distinct(Ctx* ctx, const Batch* b, Batch** out);
 int32_t op_semijoin(Ctx* ctx, const Batch* pairs, const Batch* keys, Batch** out);
 int32_t op_window_delta(Ctx* ctx, const Spine* trace, const Batch* delta, int has_prev, const u64* s0, const u64* e0,
                         const u64* s1, const u64* e1, Batch** out);
-int32_t op_map_index(Ctx* ctx, const Batch* b, const dbsp_proj* proj, Batch** out);
+template <class F>
+int32_t op_map_index(Ctx* ctx, const Batch* b, const F* proj, Batch** out);
 int32_t op_shard_partition(Ctx* ctx, const Batch* b, u32 P, Batch** outs);
 int32_t batch_build_csr(Ctx* ctx, Batch* b);
 int32_t batch_lower_bound(Ctx* ctx, const Batch* b, const u64* key, u64* pos);

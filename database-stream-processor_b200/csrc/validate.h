@@ -85,6 +85,51 @@ inline uint32_t proj_table_mask(const dbsp_proj& p) {
   return mask;
 }
 
+// Operands an instruction pops (it pushes one value; PUSH pops none)
+inline int rowfn_arity(uint8_t op) {
+  if (op == DBSP_FN_PUSH) return 0;
+  if (op <= DBSP_FN_LNOT) return 1;
+  return op == DBSP_FN_SELECT ? 3 : 2;
+}
+// A row function: the instructions fit the array, every op and PUSH source is valid for the call (lanes as in
+// valid_src), the stack never underflows or exceeds DBSP_MAX_STACK, and it ends with the output lanes + the keep flag.
+// One pass over the program, so the depth at each instruction is known before any row is evaluated.
+inline std::string valid_rowfn(const dbsp_rowfn* f, int nk, int n_lval, int n_rval, const std::string& what) {
+  if (!f) return what + ": fn is NULL";
+  std::string m = valid_schema(&f->out_schema, what, "fn.out_schema");
+  if (!m.empty()) return m;
+  if (f->n_insn > DBSP_MAX_INSNS) return what + ": fn.n_insn = " + num(f->n_insn) + " exceeds " + num(DBSP_MAX_INSNS);
+  int depth = 0;
+  for (int i = 0; i < f->n_insn; i++) {
+    const dbsp_insn& in = f->code[i];
+    const std::string where = what + ": fn.code[" + num(i) + "]";
+    if (in.op > DBSP_FN_SELECT) return where + ".op = " + num(in.op) + " is not an instruction";
+    if (in.op == DBSP_FN_PUSH) {
+      dbsp_src s;
+      s.kind = in.kind;
+      s.idx = in.idx;
+      s.cst = in.cst;
+      m = valid_src(s, nk, n_lval, n_rval, where);
+      if (!m.empty()) return m;
+    }
+    const int pops = rowfn_arity(in.op);
+    if (depth < pops) return where + ": stack underflow (depth " + num(depth) + ", the op takes " + num(pops) + ")";
+    depth += 1 - pops;
+    if (depth > DBSP_MAX_STACK) return where + ": stack deeper than " + num(DBSP_MAX_STACK);
+  }
+  const int L = f->out_schema.n_key_lanes + f->out_schema.n_val_lanes;
+  if (depth != L + 1)
+    return what + ": fn ends with stack depth " + num(depth) + ", needs " + num(L + 1) + " (the output lanes, then the keep flag)";
+  return "";
+}
+// columns of a raw table a row function reads (bit l = column l); call after valid_rowfn
+inline uint32_t rowfn_table_mask(const dbsp_rowfn& f) {
+  uint32_t mask = 0;
+  for (int i = 0; i < f.n_insn; i++)
+    if (f.code[i].op == DBSP_FN_PUSH && f.code[i].kind != DBSP_SRC_CONST) mask |= 1u << f.code[i].idx;
+  return mask;
+}
+
 // What an aggregate needs of its three operands: delta and the input trace share one schema, the output trace has
 // their key lanes, and each kind its own value shape.
 inline std::string valid_aggregate(const dbsp_schema& delta, const dbsp_schema& in, const dbsp_schema& out, int32_t kind) {

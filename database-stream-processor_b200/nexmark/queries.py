@@ -1,4 +1,4 @@
-"""Nexmark q0 / q3 / q4 / q7 on the Stream API.
+"""Nexmark q0 / q1 / q2 / q3 / q4 / q7 on the Stream API.
 
 The reference's `NexmarkStream` is one stream of `Event` enum rows
 (crates/nexmark/src/queries/mod.rs:12); here it is three column tables
@@ -15,6 +15,7 @@ from ..zset import Proj, Schema, col, key, lval, rval
 WATERMARK_INTERVAL_SECONDS = 4  # queries/mod.rs:12
 TUMBLE_SECONDS = 10             # queries/q7.rs:43
 CATEGORY_OF_INTEREST = 10       # queries/q3.rs:31
+AUCTION_ID_MODULO = 123         # queries/q2.rs:21
 
 
 @dataclass
@@ -34,6 +35,16 @@ def add_nexmark_input(circuit: RootCircuit):
 def q0(inp: NexmarkTables) -> Stream:
     """q0 pass-through of bids (queries/q0.rs): plumbing only."""
     return inp.bid.flat_map_index(Proj(Schema("uuuuu"), [col(0), col(1), col(2), col(3), col(4)]))
+
+
+def q1(inp: NexmarkTables) -> Stream:
+    """q1 currency conversion (queries/q1.rs:31-39): every bid with price * 89 / 100, in u64 arithmetic."""
+    return inp.bid.flat_map_index(Proj(Schema("uuuuu"), [col(0), col(1), (col(2) * 89).divu(100), col(3), col(4)]))
+
+
+def q2(inp: NexmarkTables) -> Stream:
+    """q2 selection (queries/q2.rs:23-31): (auction, price) of the bids whose auction % 123 == 0."""
+    return inp.bid.flat_map_index(Proj(Schema("uu"), [col(0), col(2)], where=[col(0).remu(AUCTION_ID_MODULO).eq(0)]))
 
 
 def q3(inp: NexmarkTables, states_of_interest=(1, 2, 3)) -> Stream:
@@ -89,4 +100,4 @@ def q7(inp: NexmarkTables) -> Stream:
     return max_price.join(bids_by_price, Proj(Schema("uuuuu"), [rval(0), rval(1), rval(2), rval(3), rval(4)]))
 
 
-QUERIES = {"q0": q0, "q3": q3, "q4": q4, "q7": q7}
+QUERIES = {"q0": q0, "q1": q1, "q2": q2, "q3": q3, "q4": q4, "q7": q7}

@@ -19,7 +19,7 @@ from typing import Iterable, Sequence
 import numpy as np
 
 from . import _capi as capi
-from ._capi import CApi, CExpr, CPred, CProj, CSchema, CSrc, as_u64, col_ptrs
+from ._capi import CApi, CExpr, CPred, CProj, CRowFn, CSchema, CSrc, as_u64, col_ptrs
 
 
 @dataclass(frozen=True)
@@ -62,34 +62,92 @@ class Schema:
 
 
 # ---- declarative row expressions (stand in for the Rust closures) --------
-class Src:
-    def __init__(self, kind, idx=0, cst=0):
-        self.kind, self.idx, self.cst = kind, idx, cst
+# A closure whose lanes are single operations over two sources and whose filter is at most MAX_PREDS comparisons of
+# two sources compiles to a `dbsp_proj`.  Anything else (nested arithmetic, %, abs, min/max, bitwise ops, shifts,
+# where_, comparisons used as values, predicates combined with & | ~) compiles to a `dbsp_rowfn` program.
+class Val:
+    """Operator sugar of every row value.  Nesting builds a tree (Fn); Src overrides the operators that still fit
+    one dbsp_expr."""
 
-    def c(self) -> CSrc:
-        s = CSrc()
-        s.kind, s.idx, s.cst = self.kind, self.idx, self.cst
-        return s
-
-    # arithmetic sugar -> Expr
-    def __neg__(self):
-        return Expr(capi.OP_NEG, self)
+    is_bool = False   # the value is 0 or 1 (a comparison or a logical combination of comparisons)
 
     def __add__(self, o):
-        return Expr(capi.OP_ADD, self, _src(o))
+        return Fn(capi.FN_ADD, self, o)
+
+    def __radd__(self, o):
+        return Fn(capi.FN_ADD, o, self)
 
     def __sub__(self, o):
-        return Expr(capi.OP_SUB, self, _src(o))
+        return Fn(capi.FN_SUB, self, o)
+
+    def __rsub__(self, o):
+        return Fn(capi.FN_SUB, o, self)
 
     def __mul__(self, o):
-        return Expr(capi.OP_MUL, self, _src(o))
+        return Fn(capi.FN_MUL, self, o)
+
+    def __rmul__(self, o):
+        return Fn(capi.FN_MUL, o, self)
 
     def __floordiv__(self, o):
-        return Expr(capi.OP_DIV, self, _src(o))
+        """signed, truncating (Rust `/` on i64), x // 0 = 0"""
+        return Fn(capi.FN_DIV, self, o)
 
-    # comparison sugar -> Pred (unsigned unless .signed())
+    def __mod__(self, o):
+        """signed remainder with the sign of the dividend (Rust `%` on i64), x % 0 = 0"""
+        return Fn(capi.FN_REM, self, o)
+
+    def divu(self, o):
+        return Fn(capi.FN_DIVU, self, o)
+
+    def remu(self, o):
+        return Fn(capi.FN_REMU, self, o)
+
+    def __neg__(self):
+        return Fn(capi.FN_NEG, self)
+
+    def __abs__(self):
+        return Fn(capi.FN_ABS, self)
+
+    def min(self, o):
+        """unsigned unless .signed()"""
+        return Fn(capi.FN_MINU, self, o)
+
+    def max(self, o):
+        return Fn(capi.FN_MAXU, self, o)
+
+    def __and__(self, o):
+        return Fn(capi.FN_AND, self, o)
+
+    def __rand__(self, o):
+        return Fn(capi.FN_AND, o, self)
+
+    def __or__(self, o):
+        return Fn(capi.FN_OR, self, o)
+
+    def __ror__(self, o):
+        return Fn(capi.FN_OR, o, self)
+
+    def __xor__(self, o):
+        return Fn(capi.FN_XOR, self, o)
+
+    def __rxor__(self, o):
+        return Fn(capi.FN_XOR, o, self)
+
+    def __invert__(self):
+        """logical NOT of a condition, bitwise NOT of any other value"""
+        return Fn(capi.FN_LNOT if self.is_bool else capi.FN_BNOT, self)
+
+    def __lshift__(self, o):
+        return Fn(capi.FN_SHL, self, o)
+
+    def __rshift__(self, o):
+        """logical shift; .signed() makes it arithmetic"""
+        return Fn(capi.FN_SHR, self, o)
+
+    # comparison sugar -> Pred (unsigned unless .signed()), usable as a filter and as a 0 / 1 value
     def _cmp(self, op, o):
-        return Pred(op, self, _src(o))
+        return Pred(op, self, _val(o))
 
     def eq(self, o):
         return self._cmp(capi.CMP_EQ, o)
@@ -120,8 +178,46 @@ class Src:
         return self._cmp(capi.CMP_IN, mask)
 
 
+class Src(Val):
+    def __init__(self, kind, idx=0, cst=0):
+        self.kind, self.idx, self.cst = kind, idx, cst
+
+    def c(self) -> CSrc:
+        s = CSrc()
+        s.kind, s.idx, s.cst = self.kind, self.idx, self.cst
+        return s
+
+    def emit(self, code):
+        code.append((capi.FN_PUSH, self.kind, self.idx, self.cst))
+
+    # arithmetic of two sources -> Expr (one dbsp_expr); with a tree operand -> Fn
+    def _op(self, op, o, tree_op):
+        if isinstance(o, Val) and not isinstance(o, Src):
+            return Fn(tree_op, self, o)
+        return Expr(op, self, _src(o))
+
+    def __neg__(self):
+        return Expr(capi.OP_NEG, self)
+
+    def __add__(self, o):
+        return self._op(capi.OP_ADD, o, capi.FN_ADD)
+
+    def __sub__(self, o):
+        return self._op(capi.OP_SUB, o, capi.FN_SUB)
+
+    def __mul__(self, o):
+        return self._op(capi.OP_MUL, o, capi.FN_MUL)
+
+    def __floordiv__(self, o):
+        return self._op(capi.OP_DIV, o, capi.FN_DIV)
+
+
 def _src(x):
     return x if isinstance(x, Src) else Src(capi.SRC_CONST, 0, int(x))
+
+
+def _val(x):
+    return x if isinstance(x, Val) else Src(capi.SRC_CONST, 0, int(x))
 
 
 def key(i):
@@ -144,7 +240,16 @@ def const(c):
     return Src(capi.SRC_CONST, 0, int(c))
 
 
-class Expr:
+def where_(c, a, b):
+    """`if c { a } else { b }` (c non-zero = true)"""
+    return Fn(capi.FN_SELECT, c, a, b)
+
+
+_EXPR_FN = {capi.OP_NEG: capi.FN_NEG, capi.OP_ADD: capi.FN_ADD, capi.OP_SUB: capi.FN_SUB, capi.OP_MUL: capi.FN_MUL,
+            capi.OP_DIV: capi.FN_DIV}
+
+
+class Expr(Val):
     def __init__(self, op, a, b=None):
         self.op, self.a, self.b = op, a, b if b is not None else Src(capi.SRC_CONST)
 
@@ -153,6 +258,13 @@ class Expr:
         e.op, e.a, e.b = self.op, self.a.c(), self.b.c()
         return e
 
+    def emit(self, code):
+        self.a.emit(code)
+        if self.op >= capi.OP_ADD:
+            self.b.emit(code)
+        if self.op != capi.OP_COPY:
+            code.append((_EXPR_FN[self.op], 0, 0, 0))
+
 
 def _expr(x) -> Expr:
     if isinstance(x, Expr):
@@ -160,26 +272,107 @@ def _expr(x) -> Expr:
     return Expr(capi.OP_COPY, _src(x))
 
 
-class Pred:
+def _lane(x):
+    """an output lane: an Expr when it fits one dbsp_expr, else the tree"""
+    if isinstance(x, Expr) or not isinstance(x, Val) or isinstance(x, Src):
+        return _expr(x)
+    return x
+
+
+_CMP_FN = {capi.CMP_EQ: (capi.FN_EQ, capi.FN_EQ), capi.CMP_NE: (capi.FN_NE, capi.FN_NE),
+           capi.CMP_LT: (capi.FN_LTU, capi.FN_LT), capi.CMP_LE: (capi.FN_LEU, capi.FN_LE),
+           capi.CMP_GT: (capi.FN_GTU, capi.FN_GT), capi.CMP_GE: (capi.FN_GEU, capi.FN_GE),
+           capi.CMP_IN: (capi.FN_IN, capi.FN_IN)}
+
+
+class Pred(Val):
+    is_bool = True
+
     def __init__(self, cmp, a, b, is_signed=False):
         self.cmp, self.a, self.b, self.is_signed = cmp, a, b, is_signed
 
     def signed(self):
         return Pred(self.cmp, self.a, self.b, True)
 
+    def fits(self):
+        return isinstance(self.a, Src) and isinstance(self.b, Src)
+
     def c(self) -> CPred:
         p = CPred()
         p.cmp, p.is_signed, p.a, p.b = self.cmp, int(self.is_signed), self.a.c(), self.b.c()
         return p
 
+    def emit(self, code):
+        self.a.emit(code)
+        self.b.emit(code)
+        code.append((_CMP_FN[self.cmp][int(self.is_signed)], 0, 0, 0))
+
+
+_BOOL_FN = {capi.FN_LNOT, capi.FN_EQ, capi.FN_NE, capi.FN_LT, capi.FN_LE, capi.FN_GT, capi.FN_GE, capi.FN_LTU,
+            capi.FN_LEU, capi.FN_GTU, capi.FN_GEU, capi.FN_IN}
+_SIGNED_FN = {capi.FN_MINU: capi.FN_MIN, capi.FN_MAXU: capi.FN_MAX, capi.FN_SHR: capi.FN_SAR}
+
+
+class Fn(Val):
+    """An expression tree node: a row-function instruction over its operand trees."""
+
+    def __init__(self, op, *args):
+        self.op, self.args = op, [_val(a) for a in args]
+        self.is_bool = op in _BOOL_FN or (op in (capi.FN_AND, capi.FN_OR) and all(a.is_bool for a in self.args)) or (
+            op == capi.FN_SELECT and self.args[1].is_bool and self.args[2].is_bool)
+
+    def signed(self):
+        """min / max / >> in their signed forms"""
+        assert self.op in _SIGNED_FN, "only min, max and >> have a signed form"
+        return Fn(_SIGNED_FN[self.op], *self.args)
+
+    def emit(self, code):
+        for a in self.args:
+            a.emit(code)
+        code.append((self.op, 0, 0, 0))
+
+
+def _i64(c):
+    c = int(c) & ((1 << 64) - 1)
+    return c - (1 << 64) if c >= 1 << 63 else c
+
+
+def compile_rowfn(schema: Schema, out: Sequence, where: Sequence = ()) -> CRowFn:
+    """The postfix program of a closure: the output lanes in order, then the keep flag (the AND of `where`)."""
+    code = []
+    for o in out:
+        _val(o).emit(code)
+    conds = [_val(w) for w in where]
+    if not conds:
+        code.append((capi.FN_PUSH, capi.SRC_CONST, 0, 1))
+    for i, w in enumerate(conds):
+        w.emit(code)
+        if not w.is_bool:
+            code += [(capi.FN_PUSH, capi.SRC_CONST, 0, 0), (capi.FN_NE, 0, 0, 0)]
+        if i:
+            code.append((capi.FN_AND, 0, 0, 0))
+    if len(code) > capi.MAX_INSNS:
+        raise ValueError(f"the closure needs {len(code)} instructions; a row function has at most {capi.MAX_INSNS}")
+    f = CRowFn()
+    f.out_schema = schema.c()
+    f.n_insn = len(code)
+    for i, (op, kind, idx, cst) in enumerate(code):
+        f.code[i].op, f.code[i].kind, f.code[i].idx, f.code[i].cst = op, kind, idx, _i64(cst)
+    return f
+
 
 class Proj:
-    """join_func / flat_map closure: output lanes + conjunctive filter."""
+    """join_func / flat_map closure: output lanes + filter.  A `dbsp_proj` when it fits one (lanes of one operation
+    over two sources, at most MAX_PREDS comparisons of two sources, AND-ed), else a `dbsp_rowfn` (is_fn)."""
 
-    def __init__(self, schema: Schema, out: Sequence, where: Sequence[Pred] = ()):
+    def __init__(self, schema: Schema, out: Sequence, where: Sequence = ()):
         assert len(out) == schema.nl, "one expression per output lane"
-        assert len(where) <= capi.MAX_PREDS
-        self.schema, self.out, self.where = schema, [_expr(o) for o in out], list(where)
+        self.schema, self.out, self.where = schema, [_lane(o) for o in out], list(where)
+        self.is_fn = not (all(isinstance(e, Expr) for e in self.out) and len(self.where) <= capi.MAX_PREDS
+                          and all(isinstance(w, Pred) and w.fits() for w in self.where))
+        if self.is_fn:
+            self._c = compile_rowfn(schema, self.out, self.where)
+            return
         p = CProj()
         p.out_schema = schema.c()
         p.n_pred = len(self.where)
@@ -191,6 +384,24 @@ class Proj:
 
     def c(self):
         return C.byref(self._c)
+
+    def as_rowfn(self) -> "Proj":
+        """The same closure compiled to a row function, whether or not it fits a dbsp_proj."""
+        p = Proj.__new__(Proj)
+        p.schema, p.out, p.where, p.is_fn = self.schema, self.out, self.where, True
+        p._c = compile_rowfn(self.schema, self.out, self.where)
+        return p
+
+
+def _factor(f):
+    """weigh's f(k,v): a value (a dbsp_expr when it fits one) or a one-lane Proj, whose filter drops rows"""
+    if isinstance(f, Proj):
+        assert f.schema.nl == 1, "a weigh factor has one lane"
+        return "weigh_fn", f.as_rowfn()._c if not f.is_fn else f._c
+    e = _lane(f)
+    if isinstance(e, Expr):
+        return "weigh", e.c()
+    return "weigh_fn", compile_rowfn(Schema("u"), [e])
 
 
 class Batch:
@@ -472,6 +683,11 @@ def _wrap(x):
     return int(x) & ((1 << 64) - 1)
 
 
+def _fn(call, proj: Proj):
+    """the entry point for the closure's form: `call` for a dbsp_proj, `call_fn` for a dbsp_rowfn"""
+    return call + "_fn" if proj.is_fn else call
+
+
 def _lanes(vals: Sequence[int] | None):
     if vals is None:
         return None
@@ -581,7 +797,7 @@ class Backend:
         else:
             wptr = weights
         out = self._out()
-        self.api.call("batch_from_table", self.ctx, col_ptrs(cols), len(cols), wptr, n, int(on_device), proj.c(), C.byref(out))
+        self.api.call(_fn("batch_from_table", proj), self.ctx, col_ptrs(cols), len(cols), wptr, n, int(on_device), proj.c(), C.byref(out))
         return Batch(self, out.value, proj.schema)
 
     def upload_begin(self, cols: Sequence, col_mask: int = 0xFF, weights=None):
@@ -597,11 +813,11 @@ class Backend:
 
     def batch_from_upload(self, up: "Upload", proj: Proj) -> Batch:
         out = self._out()
-        self.api.call("batch_from_upload", self.ctx, up.h, proj.c(), C.byref(out))
+        self.api.call(_fn("batch_from_upload", proj), self.ctx, up.h, proj.c(), C.byref(out))
         return Batch(self, out.value, proj.schema)
 
     def proj_table_mask(self, proj: Proj) -> int:
-        return int(self.api._proj_table_mask(proj.c()))
+        return int((self.api._rowfn_table_mask if proj.is_fn else self.api._proj_table_mask)(proj.c()))
 
     def batch_from_sorted(self, schema: Schema, cols: Sequence, weights, n: int, on_device: bool) -> Batch:
         out = self._out()
@@ -652,12 +868,12 @@ class Backend:
     # -- operators ---------------------------------------------------------
     def join_delta_trace(self, delta: Batch, trace: Spine, proj: Proj, delta_is_left=True) -> Batch:
         out = self._out()
-        self.api.call("join_delta_trace", self.ctx, delta.h, trace.h, proj.c(), int(delta_is_left), C.byref(out))
+        self.api.call(_fn("join_delta_trace", proj), self.ctx, delta.h, trace.h, proj.c(), int(delta_is_left), C.byref(out))
         return Batch(self, out.value, proj.schema)
 
     def join_batches(self, left: Batch, right: Batch, proj: Proj) -> Batch:
         out = self._out()
-        self.api.call("join_batches", self.ctx, left.h, right.h, proj.c(), C.byref(out))
+        self.api.call(_fn("join_batches", proj), self.ctx, left.h, right.h, proj.c(), C.byref(out))
         return Batch(self, out.value, proj.schema)
 
     def semijoin(self, pairs: Batch, keys: Batch) -> Batch:
@@ -671,9 +887,10 @@ class Backend:
         return Batch(self, out.value, out_trace.schema)
 
     def weigh(self, b: Batch, f, mode: int) -> Batch:
+        """f: a value of the key / value lanes, or a one-lane Proj whose filter drops rows."""
         out = self._out()
-        e = _expr(f).c()
-        self.api.call("weigh", self.ctx, b.h, C.byref(e), mode, C.byref(out))
+        call, e = _factor(f)
+        self.api.call(call, self.ctx, b.h, C.byref(e), mode, C.byref(out))
         return Batch(self, out.value)
 
     def distinct_delta(self, delta: Batch, integral: Spine) -> Batch:
@@ -697,7 +914,7 @@ class Backend:
 
     def map_index(self, b: Batch, proj: Proj) -> Batch:
         out = self._out()
-        self.api.call("map_index", self.ctx, b.h, proj.c(), C.byref(out))
+        self.api.call(_fn("map_index", proj), self.ctx, b.h, proj.c(), C.byref(out))
         return Batch(self, out.value, proj.schema)
 
     def shard_partition(self, b: Batch, n_shards: int):

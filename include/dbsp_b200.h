@@ -26,7 +26,11 @@
  * that a comment below does not call optional; a schema without 1..8 lanes
  * or with a lane type other than DBSP_U64 / DBSP_I64; a row expression whose
  * kind / op / cmp is outside its enum, whose n_pred exceeds DBSP_MAX_PREDS or
- * whose idx is not below the lane count of the source it names; two operands
+ * whose idx is not below the lane count of the source it names; a row
+ * function with more than DBSP_MAX_INSNS instructions, an op or a PUSH kind
+ * outside its enum, a PUSH idx not below the lane count of its source, a stack
+ * that underflows or grows past DBSP_MAX_STACK, or a final depth other than
+ * the output lanes + 1 (checked in O(n_insn)); two operands
  * whose schemas do not fit each other (noted per call).  DESIGN.md §1 lists
  * the checks of every entry point.
  *
@@ -122,6 +126,48 @@ typedef struct dbsp_proj {
   dbsp_pred pred[DBSP_MAX_PREDS];
 } dbsp_proj;
 
+/* Row functions: closures that are expression trees (nested arithmetic, remainders, bitwise ops, conditionals,
+ * predicates combined with AND / OR / NOT), the second closure form, accepted by the `_fn` twins of the calls that
+ * take a dbsp_proj.  A program is postfix over a stack of u64 values, at most DBSP_MAX_STACK deep: PUSH pushes the
+ * source `kind` / `idx` / `cst` (the meaning of dbsp_src); every other instruction pops its operands (the last
+ * pushed is the right-hand one) and pushes one result, and ignores kind, idx and cst.  When the program ends the
+ * stack holds exactly L + 1 values, L = the lane count of out_schema: the output lanes in order, then the keep
+ * flag (non-zero = keep the row).  Every operation is total (wrapping, no trap).  DESIGN.md §2 defines them. */
+#define DBSP_MAX_INSNS 64
+#define DBSP_MAX_STACK 16
+enum dbsp_fn_op {
+  DBSP_FN_PUSH = 0,
+  /* unary */
+  DBSP_FN_NEG = 1, DBSP_FN_ABS = 2 /* wrapping_abs: ABS(MIN) = MIN */, DBSP_FN_BNOT = 3, DBSP_FN_LNOT = 4 /* x == 0 */,
+  /* binary */
+  DBSP_FN_ADD = 5, DBSP_FN_SUB = 6, DBSP_FN_MUL = 7,
+  DBSP_FN_DIV = 8, DBSP_FN_REM = 9,    /* signed, wrapping: x / 0 = x % 0 = 0, MIN / -1 = MIN, MIN % -1 = 0 */
+  DBSP_FN_DIVU = 10, DBSP_FN_REMU = 11, /* u64: x / 0 = x % 0 = 0 */
+  DBSP_FN_MIN = 12, DBSP_FN_MAX = 13, DBSP_FN_MINU = 14, DBSP_FN_MAXU = 15,
+  DBSP_FN_AND = 16, DBSP_FN_OR = 17, DBSP_FN_XOR = 18,
+  DBSP_FN_SHL = 19, DBSP_FN_SHR = 20, DBSP_FN_SAR = 21, /* count mod 64 (wrapping_shl / _shr) */
+  /* comparisons: 0 or 1 */
+  DBSP_FN_EQ = 22, DBSP_FN_NE = 23,
+  DBSP_FN_LT = 24, DBSP_FN_LE = 25, DBSP_FN_GT = 26, DBSP_FN_GE = 27,     /* signed   */
+  DBSP_FN_LTU = 28, DBSP_FN_LEU = 29, DBSP_FN_GTU = 30, DBSP_FN_GEU = 31, /* unsigned */
+  DBSP_FN_IN = 32,    /* a < 64 && bit a of b is set (DBSP_CMP_IN) */
+  /* ternary */
+  DBSP_FN_SELECT = 33 /* c, a, b -> c != 0 ? a : b */
+};
+typedef struct dbsp_insn {
+  uint8_t op;   /* dbsp_fn_op */
+  uint8_t kind; /* PUSH: dbsp_src_kind */
+  uint8_t idx;  /* PUSH: lane / column */
+  uint8_t pad_[5];
+  int64_t cst;  /* PUSH of DBSP_SRC_CONST */
+} dbsp_insn;
+typedef struct dbsp_rowfn {
+  dbsp_schema out_schema;
+  uint8_t n_insn;
+  uint8_t pad_[5];
+  dbsp_insn code[DBSP_MAX_INSNS];
+} dbsp_rowfn;
+
 /* Aggregators (operator/aggregate/{max,min,fold}.rs, mod.rs:129-156). */
 enum dbsp_agg_kind {
   DBSP_AGG_MAX = 0,        /* Max over the value tuple  (max.rs:36-55)       */
@@ -206,6 +252,14 @@ int32_t dbsp_upload_free(dbsp_upload* up);
 /* Columns of the table a projection reads (bit l = a source with idx l);
  * 0 for a NULL or malformed projection.  Needs no context. */
 uint32_t dbsp_proj_table_mask(const dbsp_proj* proj);
+/* The same three calls with a row function (dbsp_rowfn) as the closure. */
+int32_t dbsp_batch_from_table_fn(dbsp_ctx* ctx, const uint64_t* const* cols,
+                                 uint32_t n_cols, const int64_t* weights,
+                                 uint64_t n, int32_t on_device,
+                                 const dbsp_rowfn* fn, dbsp_batch** out);
+int32_t dbsp_batch_from_upload_fn(dbsp_ctx* ctx, dbsp_upload* up,
+                                  const dbsp_rowfn* fn, dbsp_batch** out);
+uint32_t dbsp_rowfn_table_mask(const dbsp_rowfn* fn);
 int32_t dbsp_batch_empty(dbsp_ctx* ctx, const dbsp_schema* schema,
                          dbsp_batch** out);
 /* Batch::merge / Merger::work run to completion (trace/mod.rs:371-396;
@@ -354,6 +408,14 @@ int32_t dbsp_join_delta_trace(dbsp_ctx* ctx, const dbsp_batch* delta,
 int32_t dbsp_join_batches(dbsp_ctx* ctx, const dbsp_batch* left,
                           const dbsp_batch* right, const dbsp_proj* proj,
                           dbsp_batch** out);
+/* Both joins with a row function as join_func; a row whose keep flag is 0
+ * is dropped. */
+int32_t dbsp_join_delta_trace_fn(dbsp_ctx* ctx, const dbsp_batch* delta,
+                                 const dbsp_spine* trace, const dbsp_rowfn* fn,
+                                 int32_t delta_is_left, dbsp_batch** out);
+int32_t dbsp_join_batches_fn(dbsp_ctx* ctx, const dbsp_batch* left,
+                             const dbsp_batch* right, const dbsp_rowfn* fn,
+                             dbsp_batch** out);
 /* SemiJoinStream::eval (operator/semijoin.rs:100-142).  `keys` has the key
  * lanes of `pairs` and no value lanes. */
 int32_t dbsp_semijoin(dbsp_ctx* ctx, const dbsp_batch* pairs,
@@ -375,6 +437,11 @@ int32_t dbsp_aggregate_delta(dbsp_ctx* ctx, const dbsp_batch* delta,
  * `mode` is a dbsp_weigh_mode; WEIGH_AVG adds a key lane (at most 7 before). */
 int32_t dbsp_weigh(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_expr* f,
                    int32_t mode, dbsp_batch** out);
+/* weigh with a row function: fn->out_schema has one lane, the factor f(k,v);
+ * a row whose keep flag is 0 contributes nothing (in WEIGH_AVG mode neither
+ * to the sum nor to the count). */
+int32_t dbsp_weigh_fn(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_rowfn* fn,
+                      int32_t mode, dbsp_batch** out);
 /* DistinctIncrementalTotal::eval (operator/distinct.rs:196-254).  delta and
  * the integral have one schema. */
 int32_t dbsp_distinct_delta(dbsp_ctx* ctx, const dbsp_batch* delta,
@@ -394,6 +461,8 @@ int32_t dbsp_window_delta(dbsp_ctx* ctx, const dbsp_spine* trace,
 /* Map/FlatMap/Index::eval + from_tuples (filter_map.rs:563-577,700-724). */
 int32_t dbsp_map_index(dbsp_ctx* ctx, const dbsp_batch* b,
                        const dbsp_proj* proj, dbsp_batch** out);
+int32_t dbsp_map_index_fn(dbsp_ctx* ctx, const dbsp_batch* b,
+                          const dbsp_rowfn* fn, dbsp_batch** out);
 /* shard_batch (operator/communication/shard.rs:165-199): split by
  * hash(key) % n_shards into n_shards (1..64) ordered batches.  The exchange itself
  * (exchange.rs:128-200) is done by the host with its collective library on

@@ -1,0 +1,240 @@
+// rowfn_oracle.cpp — the CPU oracle with row functions (dbsp_rowfn, include/dbsp_b200.h): the whole oracle of
+// oracle/dbsp_oracle.cpp, unchanged, plus the `_fn` entry points, in one translation unit so that they build on its
+// batches, traces, consolidation and error text.  The oracle's own library stays the checker of every `dbsp_proj`
+// test; this one (libdbsp_oracle_fn.so, test infrastructure like it, never linked into the product) is the checker
+// of the row-function tests.  The interpreter below is written apart from the CUDA library's; validate.h is shared,
+// so both libraries refuse the same programs with the same texts.
+#include "../oracle/dbsp_oracle.cpp"
+
+namespace {
+
+// The postfix program over a stack; afterwards st[0..L) are the output lanes and st[L] the keep flag.  The arithmetic
+// follows Rust's wrapping_* integer methods with x / 0 = x % 0 = 0 (DESIGN §2).
+void run_rowfn(const dbsp_rowfn& f, const Env& e, u64* st) {
+  int sp = 0;
+  for (int pc = 0; pc < f.n_insn; pc++) {
+    const dbsp_insn& in = f.code[pc];
+    if (in.op == DBSP_FN_PUSH) {
+      dbsp_src s;
+      s.kind = in.kind;
+      s.idx = in.idx;
+      s.cst = in.cst;
+      st[sp++] = src_val(s, e);
+      continue;
+    }
+    const int pops = dbsp_validate::rowfn_arity(in.op);
+    const u64 a = st[sp - pops], b = pops >= 2 ? st[sp - pops + 1] : 0, c = pops == 3 ? st[sp - 1] : 0;
+    const i64 sa = (i64)a, sb = (i64)b;
+    u64 r = 0;
+    switch (in.op) {
+      case DBSP_FN_NEG: r = (u64)0 - a; break;
+      case DBSP_FN_ABS: r = sa < 0 ? (u64)0 - a : a; break;
+      case DBSP_FN_BNOT: r = ~a; break;
+      case DBSP_FN_LNOT: r = a == 0; break;
+      case DBSP_FN_ADD: r = a + b; break;
+      case DBSP_FN_SUB: r = a - b; break;
+      case DBSP_FN_MUL: r = a * b; break;
+      case DBSP_FN_DIV: r = sb == 0 ? 0 : sb == -1 ? (u64)0 - a : (u64)(sa / sb); break;   // MIN / -1 would trap
+      case DBSP_FN_REM: r = (sb == 0 || sb == -1) ? 0 : (u64)(sa % sb); break;
+      case DBSP_FN_DIVU: r = b == 0 ? 0 : a / b; break;
+      case DBSP_FN_REMU: r = b == 0 ? 0 : a % b; break;
+      case DBSP_FN_MIN: r = (u64)std::min(sa, sb); break;
+      case DBSP_FN_MAX: r = (u64)std::max(sa, sb); break;
+      case DBSP_FN_MINU: r = std::min(a, b); break;
+      case DBSP_FN_MAXU: r = std::max(a, b); break;
+      case DBSP_FN_AND: r = a & b; break;
+      case DBSP_FN_OR: r = a | b; break;
+      case DBSP_FN_XOR: r = a ^ b; break;
+      case DBSP_FN_SHL: r = a << (b % 64); break;
+      case DBSP_FN_SHR: r = a >> (b % 64); break;
+      case DBSP_FN_SAR: r = (u64)(sa >> (b % 64)); break;
+      case DBSP_FN_EQ: r = a == b; break;
+      case DBSP_FN_NE: r = a != b; break;
+      case DBSP_FN_LT: r = sa < sb; break;
+      case DBSP_FN_LE: r = sa <= sb; break;
+      case DBSP_FN_GT: r = sa > sb; break;
+      case DBSP_FN_GE: r = sa >= sb; break;
+      case DBSP_FN_LTU: r = a < b; break;
+      case DBSP_FN_LEU: r = a <= b; break;
+      case DBSP_FN_GTU: r = a > b; break;
+      case DBSP_FN_GEU: r = a >= b; break;
+      case DBSP_FN_IN: r = a < 64 && ((b >> a) & 1); break;
+      case DBSP_FN_SELECT: r = a != 0 ? b : c; break;
+    }
+    sp -= pops;
+    st[sp++] = r;
+  }
+}
+// the output row and whether the program keeps it
+bool project_fn(const dbsp_rowfn& f, const Env& e, u64* row) {
+  u64 st[DBSP_MAX_STACK];
+  run_rowfn(f, e, st);
+  const int nl = f.out_schema.n_key_lanes + f.out_schema.n_val_lanes;
+  for (int l = 0; l < nl; l++) row[l] = st[l];
+  return st[nl] != 0;
+}
+
+// Join::eval (operator/join.rs:436-473) with a row function as join_func: the merge walk of join_into.
+void join_into_fn(const Batch& L, const Batch& R, const dbsp_rowfn& f, bool swap, Tuples& out) {
+  size_t i = 0, j = 0;
+  u64 key[MAXL], v1[MAXL], v2[MAXL], row[MAXL];
+  while (i < L.K.n && j < R.K.n) {
+    int c = cmp_rows(L.K, i, R.K, j);
+    if (c < 0) { i = i + advance(i, L.K.n, [&](size_t x) { return cmp_rows(L.K, x, R.K, j) < 0; }); }
+    else if (c > 0) { j = j + advance(j, R.K.n, [&](size_t x) { return cmp_rows(R.K, x, L.K, i) < 0; }); }
+    else {
+      L.K.get(i, key);
+      size_t l0, l1, r0, r1;
+      L.vrange(i, l0, l1);
+      R.vrange(j, r0, r1);
+      for (size_t a = l0; a < l1; a++) {
+        if (L.indexed()) L.V.get(a, v1);
+        for (size_t b = r0; b < r1; b++) {
+          if (R.indexed()) R.V.get(b, v2);
+          Env e = swap ? Env{key, v2, v1} : Env{key, v1, v2};
+          if (project_fn(f, e, row)) out.push(row, (i64)((u64)L.w[a] * (u64)R.w[b]));
+        }
+      }
+      i++; j++;
+    }
+  }
+}
+
+int32_t table_to_batch_fn(const char* what, const u64* const* cols, uint32_t ncols, unsigned col_mask, const i64* w, u64 n,
+                          const dbsp_rowfn* fn, orc_batch** out) {
+  REFUSE(dv::valid_rowfn(fn, (int)ncols, (int)ncols, (int)ncols, what));
+  const unsigned used = dv::rowfn_table_mask(*fn);
+  CHECK_ARG((used & ~col_mask) == 0, std::string(what) + ": fn reads column " + std::to_string(__builtin_ctz((used & ~col_mask) | 0x100u)) +
+                                         ", which col_mask left out of the upload");
+  REFUSE(valid_cols(what, cols, (int)ncols, n, used));
+  Tuples t(fn->out_schema);
+  u64 lv[MAXL] = {0}, row[MAXL];
+  for (u64 i = 0; i < n; i++) {
+    for (uint32_t c = 0; c < ncols; c++) if ((used >> c) & 1) lv[c] = cols[c][i];
+    Env e{lv, lv, lv};
+    if (project_fn(*fn, e, row)) t.push(row, w ? w[i] : 1);
+  }
+  *out = wrap(t.build());
+  return DBSP_OK;
+}
+
+std::string valid_join_fn(const char* what, const dbsp_schema& left, const dbsp_schema& right, const dbsp_rowfn* f) {
+  if (!dv::same_key_lanes(left, right)) return std::string(what) + ": the two inputs differ in key lanes (count or type)";
+  return dv::valid_rowfn(f, left.n_key_lanes, left.n_val_lanes, right.n_val_lanes, what);
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t orc_batch_from_table_fn(orc_ctx* c, const u64* const* cols, uint32_t ncols, const i64* w, u64 n, int32_t,
+                                const dbsp_rowfn* fn, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  CHECK_ARG(ncols >= 1 && ncols <= MAXL, "batch_from_table_fn: n_cols = " + std::to_string(ncols) + ": a table has 1..8 columns");
+  ROWS32(n);
+  return table_to_batch_fn(WHAT, cols, ncols, ~0u, w, n, fn, out);
+}
+
+int32_t orc_batch_from_upload_fn(orc_ctx* c, orc_upload* u, const dbsp_rowfn* fn, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(u, "upload");
+  return table_to_batch_fn(WHAT, u->cols, u->n_cols, u->col_mask, u->w, u->n, fn, out);
+}
+
+uint32_t orc_rowfn_table_mask(const dbsp_rowfn* fn) {
+  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "rowfn_table_mask").empty()) return 0;
+  return dv::rowfn_table_mask(*fn);
+}
+
+// JoinTrace::eval with Time = () (operator/join.rs:732-863): delta joined with every batch of the trace.
+int32_t orc_join_delta_trace_fn(orc_ctx* c, const orc_batch* delta, const orc_spine* tr, const dbsp_rowfn* fn,
+                                int32_t delta_is_left, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(delta, "delta");
+  NOT_NULL(tr, "trace");
+  REFUSE(delta_is_left ? valid_join_fn(WHAT, delta->p->s, tr->s.s, fn) : valid_join_fn(WHAT, tr->s.s, delta->p->s, fn));
+  Tuples t(fn->out_schema);
+  for (auto& b : tr->s.batches) join_into_fn(*delta->p, *b, *fn, !delta_is_left, t);
+  *out = wrap(t.build());
+  return DBSP_OK;
+}
+
+int32_t orc_join_batches_fn(orc_ctx* c, const orc_batch* l, const orc_batch* r, const dbsp_rowfn* fn, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(l, "left");
+  NOT_NULL(r, "right");
+  REFUSE(valid_join_fn(WHAT, l->p->s, r->p->s, fn));
+  Tuples t(fn->out_schema);
+  join_into_fn(*l->p, *r->p, *fn, false, t);
+  *out = wrap(t.build());
+  return DBSP_OK;
+}
+
+// weigh (operator/aggregate/mod.rs:297-323) with a one-lane row function: a row the program drops adds nothing to
+// the sum, nor (WEIGH_AVG) to the count.
+int32_t orc_weigh_fn(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* f, int32_t mode, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  const Batch& B = *b->p;
+  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || mode == DBSP_WEIGH_AVG, "weigh_fn: mode = " + std::to_string(mode) + " is not a weigh mode");
+  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || B.s.n_key_lanes < MAXL, "weigh_fn: WEIGH_AVG adds a key lane and the batch already has 8");
+  CHECK_ARG(mode == DBSP_WEIGH_AVG || B.s.n_key_lanes >= 1, "weigh_fn: WEIGH_LINEAR of a batch without key lanes has no output lanes");
+  REFUSE(dv::valid_rowfn(f, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, WHAT));
+  CHECK_ARG(f->out_schema.n_key_lanes + f->out_schema.n_val_lanes == 1, "weigh_fn: fn.out_schema must have one lane (the factor)");
+  dbsp_schema s = B.s;
+  s.n_val_lanes = 0;
+  if (mode == DBSP_WEIGH_AVG) { s.lane_types[s.n_key_lanes] = DBSP_U64; s.n_key_lanes++; }
+  Builder bld(s);
+  u64 key[MAXL], val[MAXL] = {0}, fv;
+  for (size_t k = 0; k < B.K.n; k++) {
+    B.K.get(k, key);
+    size_t lo, hi;
+    B.vrange(k, lo, hi);
+    i64 agg = 0, cnt = 0;
+    for (size_t v = lo; v < hi; v++) {
+      if (B.indexed()) B.V.get(v, val);
+      Env e{key, val, val};
+      if (!project_fn(*f, e, &fv)) continue;
+      agg = (i64)((u64)agg + fv * (u64)B.w[v]);
+      cnt = (i64)((u64)cnt + (u64)B.w[v]);
+    }
+    if (mode == DBSP_WEIGH_AVG) {
+      key[B.s.n_key_lanes] = 0; if (agg != 0) bld.push(key, nullptr, agg);
+      key[B.s.n_key_lanes] = 1; if (cnt != 0) bld.push(key, nullptr, cnt);
+    } else if (agg != 0) {
+      bld.push(key, nullptr, agg);
+    }
+  }
+  *out = wrap(bld.done());
+  return DBSP_OK;
+}
+
+// Map/FlatMap/Index::eval + from_tuples (operator/filter_map.rs:563-577,700-724).
+int32_t orc_map_index_fn(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* fn, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  const Batch& B = *b->p;
+  REFUSE(dv::valid_rowfn(fn, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, WHAT));
+  Tuples t(fn->out_schema);
+  u64 key[MAXL], val[MAXL] = {0}, row[MAXL];
+  for (size_t k = 0; k < B.K.n; k++) {
+    B.K.get(k, key);
+    size_t lo, hi;
+    B.vrange(k, lo, hi);
+    for (size_t v = lo; v < hi; v++) {
+      if (B.indexed()) B.V.get(v, val);
+      Env e{key, val, val};
+      if (project_fn(*fn, e, row)) t.push(row, B.w[v]);
+    }
+  }
+  *out = wrap(t.build());
+  return DBSP_OK;
+}
+
+}  // extern "C"

@@ -6,9 +6,11 @@ include/dbsp_b200.h (CUDA library `libdbsp_b200.so`, sm_90a).  Importable as
 """
 from . import _capi as capi
 from .circuit import FoldCount, FoldSum, Max, Min, RootCircuit, Stream
-from .zset import Backend, Batch, Batcher, Merger, Proj, Schema, Spine, col, const, key, lval, rval, val, where_
+from .zset import (Backend, Batch, Batcher, Merger, Proj, Schema, Spine, col, const, fanout_index, key, lval, rval, val,
+                   where_)
 
 __all__ = [
     "capi", "RootCircuit", "Stream", "Max", "Min", "FoldCount", "FoldSum", "Backend", "Batch", "Proj",
     "Schema", "Spine", "Batcher", "Merger", "key", "lval", "rval", "val", "col", "const", "where_",
+    "fanout_index",
 ]

@@ -14,12 +14,13 @@ MAX_LANES = 8
 MAX_PREDS = 4
 MAX_INSNS = 64
 MAX_STACK = 16
+MAX_FANOUT = 64
 
 OK = 0
 ERR_NAMES = {1: "DBSP_ERR_INVALID", 2: "DBSP_ERR_CUDA", 3: "DBSP_ERR_NO_DEVICE", 4: "DBSP_ERR_UNSUPPORTED"}
 
 U64, I64 = 0, 1
-SRC_KEY, SRC_LVAL, SRC_RVAL, SRC_CONST = 0, 1, 2, 3
+SRC_KEY, SRC_LVAL, SRC_RVAL, SRC_CONST, SRC_FANOUT = 0, 1, 2, 3, 4
 OP_COPY, OP_NEG, OP_ADD, OP_SUB, OP_MUL, OP_DIV = range(6)
 CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_IN = range(7)
 AGG_MAX, AGG_MIN, AGG_FOLD_COUNT, AGG_FOLD_SUM, AGG_WCOUNT, AGG_WCOUNT2 = range(6)
@@ -87,6 +88,8 @@ _SIGS = {
     "batch_from_upload": [_P, _P, C.POINTER(CProj), _PP],
     "batch_from_table_fn": [_P, _PP, C.c_uint32, _P, C.c_uint64, C.c_int32, C.POINTER(CRowFn), _PP],
     "batch_from_upload_fn": [_P, _P, C.POINTER(CRowFn), _PP],
+    "batch_from_table_fanout": [_P, _PP, C.c_uint32, _P, C.c_uint64, C.c_int32, C.POINTER(CRowFn), C.c_uint32, _PP],
+    "batch_from_upload_fanout": [_P, _P, C.POINTER(CRowFn), C.c_uint32, _PP],
     "upload_free": [_P],
     "batch_empty": [_P, C.POINTER(CSchema), _PP],
     "batch_merge": [_P, _P, _P, _PP],
@@ -138,6 +141,7 @@ _SIGS = {
     "window_delta": [_P, _P, _P, C.c_int32, _U64P, _U64P, _U64P, _U64P, _PP],
     "map_index": [_P, _P, C.POINTER(CProj), _PP],
     "map_index_fn": [_P, _P, C.POINTER(CRowFn), _PP],
+    "map_index_fanout": [_P, _P, C.POINTER(CRowFn), C.c_uint32, _PP],
     "shard_partition": [_P, _P, C.c_uint32, _PP],
     "comm_create": [_P, C.c_int32, C.c_int32, C.c_uint64, _P],
     "comm_connect": [_P, _P],
@@ -149,11 +153,11 @@ _SIGS = {
     "allreduce_max_u64": [_P, _U64P],
 }
 COMM_BLOB_BYTES = 128
-# The row-function entry points.  The CUDA library exports them all; the CPU oracle of the dbsp_proj tests
-# (oracle/libdbsp_oracle.so) has none, its row-function build (oracle_fn/libdbsp_oracle_fn.so) has them.  A library
-# without them binds every other call, and calling one of them raises DbspError.
+# The row-function entry points, fan-outs included.  The CUDA library exports them all; the CPU oracle of the
+# dbsp_proj tests (oracle/libdbsp_oracle.so) has none, its row-function build (oracle_fn/libdbsp_oracle_fn.so) has
+# them.  A library without them binds every other call, and calling one of them raises DbspError.
 ROWFN_CALLS = {"batch_from_table_fn", "batch_from_upload_fn", "join_delta_trace_fn", "join_batches_fn", "weigh_fn",
-               "map_index_fn"}
+               "map_index_fn", "batch_from_table_fanout", "batch_from_upload_fanout", "map_index_fanout"}
 
 
 class CApi:
@@ -179,12 +183,14 @@ class CApi:
         self._proj_table_mask = getattr(lib, prefix + "proj_table_mask")
         self._proj_table_mask.restype = C.c_uint32
         self._proj_table_mask.argtypes = [C.POINTER(CProj)]
-        if hasattr(lib, prefix + "rowfn_table_mask"):
-            self._rowfn_table_mask = getattr(lib, prefix + "rowfn_table_mask")
-            self._rowfn_table_mask.restype = C.c_uint32
-            self._rowfn_table_mask.argtypes = [C.POINTER(CRowFn)]
-        else:
-            self._rowfn_table_mask = self._not_exported(prefix + "rowfn_table_mask")
+        for mask in ("rowfn_table_mask", "fanout_table_mask"):
+            if hasattr(lib, prefix + mask):
+                fn = getattr(lib, prefix + mask)
+                fn.restype = C.c_uint32
+                fn.argtypes = [C.POINTER(CRowFn)]
+            else:
+                fn = self._not_exported(prefix + mask)
+            setattr(self, "_" + mask, fn)
 
     @staticmethod
     def _not_exported(symbol):
@@ -194,7 +200,8 @@ class CApi:
 
     @staticmethod
     def symbols(prefix: str = "dbsp_"):
-        return [prefix + n for n in list(_SIGS) + ["last_error", "ctx_stream", "proj_table_mask", "rowfn_table_mask"]]
+        return [prefix + n for n in list(_SIGS) + ["last_error", "ctx_stream", "proj_table_mask", "rowfn_table_mask",
+                                                    "fanout_table_mask"]]
 
     def check(self, rc: int, what: str):
         if rc != OK:

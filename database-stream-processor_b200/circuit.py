@@ -152,7 +152,8 @@ class TableStream:
 
     def flat_map_index(self, proj: Proj) -> "Stream":
         """flat_map_index on the event stream (filter_map.rs:143-152,700-724):
-        filter + project + from_tuples, straight from the raw columns."""
+        filter + project + from_tuples, straight from the raw columns.  A fan-out `proj` (`Proj(..., fanout=n)`)
+        yields up to n rows per event, from the table and from an upload alike."""
         be = self.circuit.be
         self.projs.append(proj)
 
@@ -211,7 +212,8 @@ class Stream:
 
     # the reference's closure-taking variants all lower to one projection + filter in the row language:
     # map / flat_map produce an OrdZSet, map_index / flat_map_index / index_with an OrdIndexedZSet — the output
-    # schema of `proj` says which (filter_map.rs:40-215, index.rs:38-62)
+    # schema of `proj` says which (filter_map.rs:40-215, index.rs:38-62).  A flat_map closure that returns several
+    # rows per input row is a fan-out `Proj(..., fanout=n)`; the backend runs it with dbsp_map_index_fanout.
     map = map_index
     flat_map = map_index
     flat_map_index = map_index

@@ -48,6 +48,18 @@ namespace dv = dbsp_validate;
       return DBSP_ERR_UNSUPPORTED;                                                               \
     }                                                                                            \
   } while (0)
+// a fan-out of n rows into n * n_out rows before consolidation: the same 32-bit bound, from the sizes alone
+#define FANOUT_ROWS(n, n_out)                                                                    \
+  do {                                                                                           \
+    const std::string m__ = dv::valid_fanout_rows((n), (n_out), WHAT);                           \
+    if (!m__.empty()) { set_error(m__); return DBSP_ERR_UNSUPPORTED; }                          \
+  } while (0)
+static RowFnFanout fanout_of(const dbsp_rowfn& fn, uint32_t n_out) {
+  RowFnFanout f;
+  static_cast<dbsp_rowfn&>(f) = fn;
+  f.n_out = n_out;
+  return f;
+}
 // host columns of a table or batch: the array and, when there are rows, each column the call reads
 static std::string valid_cols(const char* what, const u64* const* cols, int ncols, u64 n, unsigned mask = ~0u) {
   if (!cols) return std::string(what) + ": cols is NULL";
@@ -536,6 +548,26 @@ int32_t dbsp_batch_from_table_fn(dbsp_ctx* ctx, const uint64_t* const* cols, uin
   return DBSP_OK;
 }
 
+int32_t dbsp_batch_from_table_fanout(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n_cols, const int64_t* w,
+                                     uint64_t n, int32_t on_device, const dbsp_rowfn* fn, uint32_t n_out,
+                                     dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "batch_from_table_fanout: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
+  REFUSE(dv::valid_fanout(n_out, WHAT));
+  REFUSE(dv::valid_rowfn(fn, (int)n_cols, (int)n_cols, (int)n_cols, WHAT, true));
+  REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, dv::rowfn_table_mask(*fn)));
+  ROWS32(n);
+  FANOUT_ROWS(n, n_out);
+  BufP hold;
+  Cols dc;
+  const i64* dw;
+  TRY(stage_columns(ctx, cols, (int)n_cols, w, n, on_device, &hold, &dc, &dw, rowfn_used_mask(*fn, 0)));
+  Batch* b = nullptr;
+  TRY(project_and_consolidate(ctx, dc, 0, (int)n_cols, dw, n, fanout_of(*fn, n_out), &b));
+  *out = H(b);
+  return DBSP_OK;
+}
+
 struct dbsp_upload {
   Ctx* ctx;
   BufP buf;
@@ -553,6 +585,10 @@ uint32_t dbsp_proj_table_mask(const dbsp_proj* proj) {
 }
 uint32_t dbsp_rowfn_table_mask(const dbsp_rowfn* fn) {
   if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "rowfn_table_mask").empty()) return 0;
+  return dv::rowfn_table_mask(*fn);
+}
+uint32_t dbsp_fanout_table_mask(const dbsp_rowfn* fn) {
+  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "fanout_table_mask", true).empty()) return 0;
   return dv::rowfn_table_mask(*fn);
 }
 
@@ -638,6 +674,25 @@ int32_t dbsp_batch_from_upload_fn(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_rowf
   CUDA_TRY(cudaStreamWaitEvent(ctx->stream, u->done, 0));   // compute stream waits for the copy
   Batch* b = nullptr;
   TRY(project_and_consolidate(ctx, u->dc, 0, u->n_cols, u->dw, u->n, *fn, &b));
+  *out = H(b);
+  return DBSP_OK;
+}
+
+int32_t dbsp_batch_from_upload_fanout(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_rowfn* fn, uint32_t n_out,
+                                      dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(u, "upload");
+  CHECK_ARG(u->ctx == ctx, "batch_from_upload_fanout: upload belongs to another context");
+  REFUSE(dv::valid_fanout(n_out, WHAT));
+  REFUSE(dv::valid_rowfn(fn, u->n_cols, u->n_cols, u->n_cols, WHAT, true));
+  {
+    const unsigned missing = dv::rowfn_table_mask(*fn) & ~u->col_mask;
+    CHECK_ARG(missing == 0, "batch_from_upload_fanout: fn reads column " + std::to_string(__builtin_ctz(missing | 0x100u)) + ", which col_mask left out of the upload");
+  }
+  FANOUT_ROWS(u->n, n_out);
+  CUDA_TRY(cudaStreamWaitEvent(ctx->stream, u->done, 0));   // compute stream waits for the copy
+  Batch* b = nullptr;
+  TRY(project_and_consolidate(ctx, u->dc, 0, u->n_cols, u->dw, u->n, fanout_of(*fn, n_out), &b));
   *out = H(b);
   return DBSP_OK;
 }
@@ -1380,6 +1435,14 @@ int32_t dbsp_map_index_fn(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_rowfn* 
   NOT_NULL(b, "batch");
   REFUSE(dv::valid_rowfn(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT));
   OUT1(op_map_index(ctx, B(b), f, &o__)) }
+int32_t dbsp_map_index_fanout(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_rowfn* f, uint32_t n_out, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  REFUSE(dv::valid_fanout(n_out, WHAT));
+  REFUSE(dv::valid_rowfn(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT, true));
+  FANOUT_ROWS(B(b)->n, n_out);
+  const RowFnFanout fo = fanout_of(*f, n_out);
+  OUT1(op_map_index(ctx, B(b), &fo, &o__)) }
 int32_t dbsp_shard_partition(dbsp_ctx* ctx, const dbsp_batch* b, uint32_t P, dbsp_batch** outs) { ENTER(ctx);
   NOT_NULL(b, "batch");
   NOT_NULL(outs, "outs");

@@ -37,6 +37,16 @@ struct ColEnv {
   __device__ __forceinline__ u64 l(int i) const { return c.c[nk + i][row]; }
   __device__ __forceinline__ u64 r(int i) const { return c.c[nk + i][row]; }
 };
+// one run of a fan-out (dbsp_*_fanout): input row `row` of a column table, generating output j (DBSP_SRC_FANOUT)
+struct FanEnv {
+  const Cols& c;
+  int nk;
+  u64 row;
+  u64 j;
+  __device__ __forceinline__ u64 k(int i) const { return c.c[i][row]; }
+  __device__ __forceinline__ u64 l(int i) const { return c.c[nk + i][row]; }
+  __device__ __forceinline__ u64 r(int i) const { return c.c[nk + i][row]; }
+};
 template <class E>
 __device__ __forceinline__ u64 src_val(const dbsp_src& s, const E& e) {
   switch (s.kind) {
@@ -105,7 +115,11 @@ __device__ __forceinline__ void run_rowfn(const dbsp_rowfn& f, const E& e, u64* 
         case DBSP_SRC_KEY: v = e.k(in.idx); break;
         case DBSP_SRC_LVAL: v = e.l(in.idx); break;
         case DBSP_SRC_RVAL: v = e.r(in.idx); break;
-        default: v = (u64)in.cst;
+        default:
+          if constexpr (std::is_same<E, FanEnv>::value) {   // only a fan-out's environment has a j
+            if (in.kind == DBSP_SRC_FANOUT) { v = e.j; break; }
+          }
+          v = (u64)in.cst;
       }
       st[sp++] = v;
       continue;
@@ -208,6 +222,19 @@ __device__ __forceinline__ bool fn_factor(const dbsp_rowfn& f, const Env& e, u64
   return keep;
 }
 
+// The virtual rows of k_project_rows.  For dbsp_proj / dbsp_rowfn virtual row v is input row v; for a fan-out
+// (RowFnFanout) it is v = i * n_out + j, so the outputs keep the input order with j ascending inside each input row,
+// and v < 2^32 (capi.cu refuses larger fan-outs from the sizes).
+template <class F>
+__device__ __forceinline__ u64 in_row(const F&, u64 v) { return v; }
+__device__ __forceinline__ u64 in_row(const RowFnFanout& f, u64 v) { return (u32)v / f.n_out; }
+template <class F>
+__device__ __forceinline__ ColEnv row_env(const F&, const Cols& in, int nk, u64 v) { return ColEnv{in, nk, v}; }
+__device__ __forceinline__ FanEnv row_env(const RowFnFanout& f, const Cols& in, int nk, u64 v) {
+  const u32 i = (u32)v / f.n_out;
+  return FanEnv{in, nk, i, (u32)v - i * f.n_out};
+}
+
 // flat_map_index over a raw table (filter_map.rs:700-724) / map_index over a
 // batch, in one pass and order preserving: a CTA evaluates the predicates of its PROJ_ROWS rows, a decoupled
 // look-back over the CTA totals gives it its output base, and the survivors' output rows are evaluated and written
@@ -231,9 +258,9 @@ k_project_rows(Cols in, int nk_in, const i64* w, u64 n, F proj, int identity, u3
     for (int it = 0; it < PROJ_IT; it++) {
       const u64 i = base + (u64)it * TB + tid;
       if (i < n) {
-        const ColEnv e{in, nk_in, i};
+        const auto e = row_env(proj, in, nk_in, i);
         fn_emit(proj, e, nl, [&](int l, u64 v) { out.c[l][i] = v; });
-        out_w[i] = w ? w[i] : 1;
+        out_w[i] = w ? w[in_row(proj, i)] : 1;
       }
     }
     return;
@@ -247,7 +274,7 @@ k_project_rows(Cols in, int nk_in, const i64* w, u64 n, F proj, int identity, u3
     const u64 i = base_row + (u64)it * TB + tid;
     bool ok = false;
     if (i < n) {
-      const ColEnv e{in, nk_in, i};
+      const auto e = row_env(proj, in, nk_in, i);
       ok = fn_keep(proj, e);
     }
     const unsigned m = __ballot_sync(0xffffffffu, ok);
@@ -280,9 +307,9 @@ k_project_rows(Cols in, int nk_in, const i64* w, u64 n, F proj, int identity, u3
     if (!((okbits >> it) & 1)) continue;
     const u64 i = base_row + (u64)it * TB + tid;
     const u64 pos = base + s_off[it * (TB / 32) + wid] + ((rk >> (8 * it)) & 0xffu);
-    const ColEnv e{in, nk_in, i};
+    const auto e = row_env(proj, in, nk_in, i);
     fn_emit(proj, e, nl, [&](int l, u64 v) { out.c[l][pos] = v; });
-    out_w[pos] = w ? w[i] : 1;
+    out_w[pos] = w ? w[in_row(proj, i)] : 1;
   }
 }
 
@@ -1002,12 +1029,17 @@ static bool filters(const dbsp_rowfn& f) {
   return !(last.op == DBSP_FN_PUSH && last.kind == DBSP_SRC_CONST && last.cst != 0);
 }
 
-// project rows of (in cols) through proj, then consolidate.
+static u64 fan_out(const dbsp_proj&) { return 1; }
+static u64 fan_out(const dbsp_rowfn&) { return 1; }
+static u64 fan_out(const RowFnFanout& f) { return f.n_out; }
+
+// project rows of (in cols) through proj, then consolidate.  n input rows; a fan-out projects n * n_out virtual rows.
 template <class F>
-int32_t project_and_consolidate(Ctx* ctx, const Cols& in, int nk_in, int n_in_lanes, const i64* w, u64 n,
+int32_t project_and_consolidate(Ctx* ctx, const Cols& in, int nk_in, int n_in_lanes, const i64* w, u64 n_in,
                                 const F& proj, Batch** out) {
   const dbsp_schema& os = proj.out_schema;
   int Lo = os.n_key_lanes + os.n_val_lanes;
+  const u64 n = n_in * fan_out(proj);
   if (n == 0) { *out = batch_new_empty(ctx, os); return DBSP_OK; }
   ROWS32(n, "map_index / flat_map_index");
   const unsigned g = (unsigned)((n + PROJ_ROWS - 1) / PROJ_ROWS);
@@ -1029,8 +1061,9 @@ int32_t project_and_consolidate(Ctx* ctx, const Cols& in, int nk_in, int n_in_la
   TmpRows t;
   TRY(tmp_alloc(ctx, Lo, m, &t));
   {
-    // the lanes the closure names read once, the output rows written once (bound: every row survives)
-    ProfScope ps(ctx, KID_PROJECT, n * (u64)(used_lanes(proj, n_in_lanes, nk_in) + (w ? 1 : 0)) * 8 + m * (u64)(Lo + 1) * 8);
+    // the lanes the closure names read once per input row, the output rows written once (bound: every row of the
+    // fan-out survives)
+    ProfScope ps(ctx, KID_PROJECT, n_in * (u64)(used_lanes(proj, n_in_lanes, nk_in) + (w ? 1 : 0)) * 8 + m * (u64)(Lo + 1) * 8);
     k_project_rows<<<g, TB, 0, ctx->stream>>>(in, nk_in, w, n, proj, filtered ? 0 : 1, g, ticket, status, t.c, t.w, d_mw);
   }
   LAUNCH_COUNT(ctx);
@@ -1038,6 +1071,7 @@ int32_t project_and_consolidate(Ctx* ctx, const Cols& in, int nk_in, int n_in_la
 }
 template int32_t project_and_consolidate(Ctx*, const Cols&, int, int, const i64*, u64, const dbsp_proj&, Batch**);
 template int32_t project_and_consolidate(Ctx*, const Cols&, int, int, const i64*, u64, const dbsp_rowfn&, Batch**);
+template int32_t project_and_consolidate(Ctx*, const Cols&, int, int, const i64*, u64, const RowFnFanout&, Batch**);
 
 // Probe `delta` against every batch of `trace` and expand the matches.
 // proj == nullptr: gather the matching trace rows unchanged.
@@ -1497,6 +1531,7 @@ int32_t op_map_index(Ctx* ctx, const Batch* b, const F* proj, Batch** out) {
 }
 template int32_t op_map_index(Ctx*, const Batch*, const dbsp_proj*, Batch**);
 template int32_t op_map_index(Ctx*, const Batch*, const dbsp_rowfn*, Batch**);
+template int32_t op_map_index(Ctx*, const Batch*, const RowFnFanout*, Batch**);
 
 // shard_batch (operator/communication/shard.rs:165-199)
 int32_t op_shard_partition(Ctx* ctx, const Batch* b, u32 P, Batch** outs) {

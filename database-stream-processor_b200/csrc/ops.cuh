@@ -2,13 +2,20 @@
 #pragma once
 #include <algorithm>
 #include <cstring>
+#include <type_traits>
 
 #include "common.cuh"
 
 int32_t compact_ordered(Ctx* ctx, const dbsp_schema& s, const Cols& in, const i64* w, const u32* keep, u64 n, Batch** out);
 unsigned proj_used_mask(const dbsp_proj& p, int nk_in);
 unsigned rowfn_used_mask(const dbsp_rowfn& f, int nk_in);
-// The closure-taking operators, for F = dbsp_proj and F = dbsp_rowfn (weigh: dbsp_expr and dbsp_rowfn).
+// A row function run n_out times per input row (the `_fanout` calls): a third closure form of the projection, whose
+// program may push DBSP_SRC_FANOUT.  It is a dbsp_rowfn, so every helper of row functions takes it as one.
+struct RowFnFanout : dbsp_rowfn {
+  u32 n_out;
+};
+// The closure-taking operators, for F = dbsp_proj and F = dbsp_rowfn (weigh: dbsp_expr and dbsp_rowfn); the
+// projection (project_and_consolidate, op_map_index) also for F = RowFnFanout.
 template <class F>
 int32_t project_and_consolidate(Ctx* ctx, const Cols& in, int nk_in, int n_in_lanes, const i64* w, u64 n,
                                 const F& proj, Batch** out);

@@ -93,8 +93,10 @@ inline int rowfn_arity(uint8_t op) {
 }
 // A row function: the instructions fit the array, every op and PUSH source is valid for the call (lanes as in
 // valid_src), the stack never underflows or exceeds DBSP_MAX_STACK, and it ends with the output lanes + the keep flag.
-// One pass over the program, so the depth at each instruction is known before any row is evaluated.
-inline std::string valid_rowfn(const dbsp_rowfn* f, int nk, int n_lval, int n_rval, const std::string& what) {
+// One pass over the program, so the depth at each instruction is known before any row is evaluated.  `fanout`: the
+// program belongs to a `_fanout` call, where a PUSH may also take DBSP_SRC_FANOUT (j; idx and cst ignored).
+inline std::string valid_rowfn(const dbsp_rowfn* f, int nk, int n_lval, int n_rval, const std::string& what,
+                               bool fanout = false) {
   if (!f) return what + ": fn is NULL";
   std::string m = valid_schema(&f->out_schema, what, "fn.out_schema");
   if (!m.empty()) return m;
@@ -104,7 +106,7 @@ inline std::string valid_rowfn(const dbsp_rowfn* f, int nk, int n_lval, int n_rv
     const dbsp_insn& in = f->code[i];
     const std::string where = what + ": fn.code[" + num(i) + "]";
     if (in.op > DBSP_FN_SELECT) return where + ".op = " + num(in.op) + " is not an instruction";
-    if (in.op == DBSP_FN_PUSH) {
+    if (in.op == DBSP_FN_PUSH && !(fanout && in.kind == DBSP_SRC_FANOUT)) {
       dbsp_src s;
       s.kind = in.kind;
       s.idx = in.idx;
@@ -126,8 +128,21 @@ inline std::string valid_rowfn(const dbsp_rowfn* f, int nk, int n_lval, int n_rv
 inline uint32_t rowfn_table_mask(const dbsp_rowfn& f) {
   uint32_t mask = 0;
   for (int i = 0; i < f.n_insn; i++)
-    if (f.code[i].op == DBSP_FN_PUSH && f.code[i].kind != DBSP_SRC_CONST) mask |= 1u << f.code[i].idx;
+    if (f.code[i].op == DBSP_FN_PUSH && f.code[i].kind < DBSP_SRC_CONST) mask |= 1u << f.code[i].idx;
   return mask;
+}
+// A fan-out's output count: 1..DBSP_MAX_FANOUT runs of the program per input row
+inline std::string valid_fanout(uint32_t n_out, const std::string& what) {
+  if (n_out < 1 || n_out > DBSP_MAX_FANOUT)
+    return what + ": n_out = " + num(n_out) + ": a fan-out gives 1.." + num(DBSP_MAX_FANOUT) + " rows per input row";
+  return "";
+}
+// n input rows fanned out to n * n_out rows before consolidation: row indices are 32-bit on the device, so 2^32-1 or
+// more is refused (DBSP_ERR_UNSUPPORTED), from the sizes alone.  n < 2^32 and n_out <= 64: the product cannot wrap.
+inline std::string valid_fanout_rows(uint64_t n, uint32_t n_out, const std::string& what) {
+  if (n * (uint64_t)n_out >= 0xffffffffull)
+    return what + ": n * n_out = " + num(n) + " * " + num(n_out) + ": 2^32-1 or more rows before consolidation; split the input";
+  return "";
 }
 
 // What an aggregate needs of its three operands: delta and the input trace share one schema, the output trace has

@@ -1,4 +1,4 @@
-"""Nexmark q0 / q1 / q2 / q3 / q4 / q7 on the Stream API.
+"""Nexmark q0 / q1 / q2 / q3 / q4 / q7, and q5 as its SQL states it (q5_hop), on the Stream API.
 
 The reference's `NexmarkStream` is one stream of `Event` enum rows
 (crates/nexmark/src/queries/mod.rs:12); here it is three column tables
@@ -10,12 +10,14 @@ from __future__ import annotations
 from dataclasses import dataclass
 
 from ..circuit import Max, Min, RootCircuit, Stream, TableStream
-from ..zset import Proj, Schema, col, key, lval, rval
+from ..zset import Proj, Schema, col, const, fanout_index, key, lval, rval
 
 WATERMARK_INTERVAL_SECONDS = 4  # queries/mod.rs:12
 TUMBLE_SECONDS = 10             # queries/q7.rs:43
 CATEGORY_OF_INTEREST = 10       # queries/q3.rs:31
 AUCTION_ID_MODULO = 123         # queries/q2.rs:21
+HOP_SLIDE_MS = 2_000            # queries/q5.rs:24-60: HOP(dateTime, INTERVAL '2' SECOND, INTERVAL '10' SECOND)
+HOP_SIZE_MS = 10_000
 
 
 @dataclass
@@ -100,4 +102,20 @@ def q7(inp: NexmarkTables) -> Stream:
     return max_price.join(bids_by_price, Proj(Schema("uuuuu"), [rval(0), rval(1), rval(2), rval(3), rval(4)]))
 
 
-QUERIES = {"q0": q0, "q1": q1, "q2": q2, "q3": q3, "q4": q4, "q7": q7}
+def q5_hop(inp: NexmarkTables) -> Stream:
+    """The SQL of queries/q5.rs:24-60 (hot items): per HOP(dateTime, 2 s, 10 s) window, the auctions with the most
+    bids, as (auction, num).  Every window is kept (no watermark).  A row's weight is the number of windows in which
+    the auction had `num` bids and no auction had more.  (The reference's DBSP q5 uses one sliding window instead.)"""
+    last = col(3) - col(3).remu(HOP_SLIDE_MS)   # the start of the latest window that holds the bid
+    j = fanout_index()
+    # (auction, starttime) for each of the size / slide windows of a bid; no window starts below 0
+    bid_windows = inp.bid.flat_map_index(Proj(Schema("uu"), [col(0), last - j * HOP_SLIDE_MS],
+                                              where=[(j * HOP_SLIDE_MS).le(last)], fanout=HOP_SIZE_MS // HOP_SLIDE_MS))
+    counts = bid_windows.aggregate_linear(const(1))                                      # ((auction, starttime), num)
+    auction_bids = counts.map_index(Proj(Schema("u", "ui"), [key(1), key(0), lval(0)]))  # starttime -> (auction, num)
+    max_bids = counts.map_index(Proj(Schema("u", "i"), [key(1), lval(0)])).aggregate(Max)   # starttime -> maxn
+    # endtime = starttime + size, so the join on starttime is the SQL's join on both
+    return auction_bids.join(max_bids, Proj(Schema("ui"), [lval(0), lval(1)], where=[lval(1).ge(rval(0)).signed()]))
+
+
+QUERIES = {"q0": q0, "q1": q1, "q2": q2, "q3": q3, "q4": q4, "q7": q7, "q5_hop": q5_hop}

@@ -240,6 +240,11 @@ def const(c):
     return Src(capi.SRC_CONST, 0, int(c))
 
 
+def fanout_index():
+    """j, the index (0 .. fanout-1) of the output a fan-out closure is generating (`Proj(..., fanout=n)`)"""
+    return Src(capi.SRC_FANOUT)
+
+
 def where_(c, a, b):
     """`if c { a } else { b }` (c non-zero = true)"""
     return Fn(capi.FN_SELECT, c, a, b)
@@ -361,15 +366,31 @@ def compile_rowfn(schema: Schema, out: Sequence, where: Sequence = ()) -> CRowFn
     return f
 
 
+def _reads_fanout(x) -> bool:
+    if isinstance(x, Src):
+        return x.kind == capi.SRC_FANOUT
+    if isinstance(x, (Expr, Pred)):
+        return _reads_fanout(x.a) or _reads_fanout(x.b)
+    if isinstance(x, Fn):
+        return any(_reads_fanout(a) for a in x.args)
+    return False
+
+
 class Proj:
     """join_func / flat_map closure: output lanes + filter.  A `dbsp_proj` when it fits one (lanes of one operation
-    over two sources, at most MAX_PREDS comparisons of two sources, AND-ed), else a `dbsp_rowfn` (is_fn)."""
+    over two sources, at most MAX_PREDS comparisons of two sources, AND-ed), else a `dbsp_rowfn` (is_fn).
 
-    def __init__(self, schema: Schema, out: Sequence, where: Sequence = ()):
+    `fanout=n` makes it a flat_map closure that returns an iterator (filter_map.rs:124-160): the closure runs n times
+    per input row with fanout_index() = 0 .. n-1, and each run whose filter holds yields one row (is_fanout, the
+    `_fanout` entry points).  A closure with fanout 1 that never reads fanout_index() is an ordinary one."""
+
+    def __init__(self, schema: Schema, out: Sequence, where: Sequence = (), fanout: int = 1):
         assert len(out) == schema.nl, "one expression per output lane"
         self.schema, self.out, self.where = schema, [_lane(o) for o in out], list(where)
-        self.is_fn = not (all(isinstance(e, Expr) for e in self.out) and len(self.where) <= capi.MAX_PREDS
-                          and all(isinstance(w, Pred) and w.fits() for w in self.where))
+        self.fanout = int(fanout)
+        self.is_fanout = self.fanout != 1 or any(_reads_fanout(x) for x in self.out + self.where)
+        self.is_fn = self.is_fanout or not (all(isinstance(e, Expr) for e in self.out) and len(self.where) <= capi.MAX_PREDS
+                                            and all(isinstance(w, Pred) and w.fits() for w in self.where))
         if self.is_fn:
             self._c = compile_rowfn(schema, self.out, self.where)
             return
@@ -389,6 +410,7 @@ class Proj:
         """The same closure compiled to a row function, whether or not it fits a dbsp_proj."""
         p = Proj.__new__(Proj)
         p.schema, p.out, p.where, p.is_fn = self.schema, self.out, self.where, True
+        p.fanout, p.is_fanout = self.fanout, self.is_fanout
         p._c = compile_rowfn(self.schema, self.out, self.where)
         return p
 
@@ -397,6 +419,8 @@ def _factor(f):
     """weigh's f(k,v): a value (a dbsp_expr when it fits one) or a one-lane Proj, whose filter drops rows"""
     if isinstance(f, Proj):
         assert f.schema.nl == 1, "a weigh factor has one lane"
+        if f.is_fanout:
+            raise ValueError("weigh: a fan-out closure yields several rows; a weigh factor is one value per row")
         return "weigh_fn", f.as_rowfn()._c if not f.is_fn else f._c
     e = _lane(f)
     if isinstance(e, Expr):
@@ -683,9 +707,22 @@ def _wrap(x):
     return int(x) & ((1 << 64) - 1)
 
 
+_FANOUT_CALLS = {"batch_from_table", "batch_from_upload", "map_index"}
+
+
 def _fn(call, proj: Proj):
-    """the entry point for the closure's form: `call` for a dbsp_proj, `call_fn` for a dbsp_rowfn"""
+    """the entry point for the closure's form: `call` for a dbsp_proj, `call_fn` for a dbsp_rowfn, `call_fanout`
+    for a fan-out"""
+    if getattr(proj, "is_fanout", False):
+        if call not in _FANOUT_CALLS:
+            raise ValueError(f"{call}: a fan-out closure applies to flat_map / flat_map_index and tables only")
+        return call + "_fanout"
     return call + "_fn" if proj.is_fn else call
+
+
+def _closure(proj: Proj):
+    """the closure arguments of the entry point `_fn` picks: the struct, and a fan-out's n_out after it"""
+    return (proj.c(), proj.fanout) if getattr(proj, "is_fanout", False) else (proj.c(),)
 
 
 def _lanes(vals: Sequence[int] | None):
@@ -797,7 +834,8 @@ class Backend:
         else:
             wptr = weights
         out = self._out()
-        self.api.call(_fn("batch_from_table", proj), self.ctx, col_ptrs(cols), len(cols), wptr, n, int(on_device), proj.c(), C.byref(out))
+        self.api.call(_fn("batch_from_table", proj), self.ctx, col_ptrs(cols), len(cols), wptr, n, int(on_device),
+                      *_closure(proj), C.byref(out))
         return Batch(self, out.value, proj.schema)
 
     def upload_begin(self, cols: Sequence, col_mask: int = 0xFF, weights=None):
@@ -813,10 +851,12 @@ class Backend:
 
     def batch_from_upload(self, up: "Upload", proj: Proj) -> Batch:
         out = self._out()
-        self.api.call(_fn("batch_from_upload", proj), self.ctx, up.h, proj.c(), C.byref(out))
+        self.api.call(_fn("batch_from_upload", proj), self.ctx, up.h, *_closure(proj), C.byref(out))
         return Batch(self, out.value, proj.schema)
 
     def proj_table_mask(self, proj: Proj) -> int:
+        if getattr(proj, "is_fanout", False):
+            return int(self.api._fanout_table_mask(proj.c()))
         return int((self.api._rowfn_table_mask if proj.is_fn else self.api._proj_table_mask)(proj.c()))
 
     def batch_from_sorted(self, schema: Schema, cols: Sequence, weights, n: int, on_device: bool) -> Batch:
@@ -914,7 +954,7 @@ class Backend:
 
     def map_index(self, b: Batch, proj: Proj) -> Batch:
         out = self._out()
-        self.api.call(_fn("map_index", proj), self.ctx, b.h, proj.c(), C.byref(out))
+        self.api.call(_fn("map_index", proj), self.ctx, b.h, *_closure(proj), C.byref(out))
         return Batch(self, out.value, proj.schema)
 
     def shard_partition(self, b: Batch, n_shards: int):

@@ -84,7 +84,11 @@ enum dbsp_src_kind {
                          for map_index / raw tables: value lane / column    */
   DBSP_SRC_RVAL = 2,  /* lane `idx` of the right value (v2 of join_func);
                          in a call with one input: the same lanes as LVAL  */
-  DBSP_SRC_CONST = 3  /* the constant `cst`                                 */
+  DBSP_SRC_CONST = 3, /* the constant `cst`                                 */
+  DBSP_SRC_FANOUT = 4 /* row functions of the `_fanout` calls only: j, the
+                         index (0 .. n_out-1) of the output being generated;
+                         idx and cst are ignored.  Every other call refuses
+                         it as outside the enum.                            */
 };
 enum dbsp_expr_op {
   DBSP_OP_COPY = 0, DBSP_OP_NEG = 1, DBSP_OP_ADD = 2, DBSP_OP_SUB = 3,
@@ -260,6 +264,26 @@ int32_t dbsp_batch_from_table_fn(dbsp_ctx* ctx, const uint64_t* const* cols,
 int32_t dbsp_batch_from_upload_fn(dbsp_ctx* ctx, dbsp_upload* up,
                                   const dbsp_rowfn* fn, dbsp_batch** out);
 uint32_t dbsp_rowfn_table_mask(const dbsp_rowfn* fn);
+/* Fan-out (flat_map returning an iterator, filter_map.rs:124-160): the row
+ * function runs n_out times per input row, with j = 0 .. n_out-1 pushed by
+ * DBSP_SRC_FANOUT; input row i yields output j iff the keep flag of run j is
+ * non-zero.  Every output row carries the weight of its input row, and the
+ * result is consolidated like every other output.  1 <= n_out <=
+ * DBSP_MAX_FANOUT (else INVALID); rows * n_out of 2^32-1 or more is
+ * UNSUPPORTED, checked from the sizes before anything runs.  The table, upload
+ * and batch forms take what batch_from_table_fn / batch_from_upload_fn /
+ * map_index_fn take, and fanout_table_mask is rowfn_table_mask with FANOUT
+ * pushes allowed (they read no column). */
+#define DBSP_MAX_FANOUT 64
+int32_t dbsp_batch_from_table_fanout(dbsp_ctx* ctx, const uint64_t* const* cols,
+                                     uint32_t n_cols, const int64_t* weights,
+                                     uint64_t n, int32_t on_device,
+                                     const dbsp_rowfn* fn, uint32_t n_out,
+                                     dbsp_batch** out);
+int32_t dbsp_batch_from_upload_fanout(dbsp_ctx* ctx, dbsp_upload* up,
+                                      const dbsp_rowfn* fn, uint32_t n_out,
+                                      dbsp_batch** out);
+uint32_t dbsp_fanout_table_mask(const dbsp_rowfn* fn);
 int32_t dbsp_batch_empty(dbsp_ctx* ctx, const dbsp_schema* schema,
                          dbsp_batch** out);
 /* Batch::merge / Merger::work run to completion (trace/mod.rs:371-396;
@@ -463,6 +487,12 @@ int32_t dbsp_map_index(dbsp_ctx* ctx, const dbsp_batch* b,
                        const dbsp_proj* proj, dbsp_batch** out);
 int32_t dbsp_map_index_fn(dbsp_ctx* ctx, const dbsp_batch* b,
                           const dbsp_rowfn* fn, dbsp_batch** out);
+/* flat_map / flat_map_index of a batch with a fan-out (see
+ * dbsp_batch_from_table_fanout): n_out runs of fn per row, j pushed by
+ * DBSP_SRC_FANOUT. */
+int32_t dbsp_map_index_fanout(dbsp_ctx* ctx, const dbsp_batch* b,
+                              const dbsp_rowfn* fn, uint32_t n_out,
+                              dbsp_batch** out);
 /* shard_batch (operator/communication/shard.rs:165-199): split by
  * hash(key) % n_shards into n_shards (1..64) ordered batches.  The exchange itself
  * (exchange.rs:128-200) is done by the host with its collective library on

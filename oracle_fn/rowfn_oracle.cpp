@@ -1,5 +1,5 @@
 // rowfn_oracle.cpp — the CPU oracle with row functions (dbsp_rowfn, include/dbsp_b200.h): the whole oracle of
-// oracle/dbsp_oracle.cpp, unchanged, plus the `_fn` entry points, in one translation unit so that they build on its
+// oracle/dbsp_oracle.cpp, unchanged, plus the `_fn` and `_fanout` entry points, in one translation unit so that they build on its
 // batches, traces, consolidation and error text.  The oracle's own library stays the checker of every `dbsp_proj`
 // test; this one (libdbsp_oracle_fn.so, test infrastructure like it, never linked into the product) is the checker
 // of the row-function tests.  The interpreter below is written apart from the CUDA library's; validate.h is shared,
@@ -9,8 +9,9 @@
 namespace {
 
 // The postfix program over a stack; afterwards st[0..L) are the output lanes and st[L] the keep flag.  The arithmetic
-// follows Rust's wrapping_* integer methods with x / 0 = x % 0 = 0 (DESIGN §2).
-void run_rowfn(const dbsp_rowfn& f, const Env& e, u64* st) {
+// follows Rust's wrapping_* integer methods with x / 0 = x % 0 = 0 (DESIGN §2).  j: the output a fan-out generates,
+// pushed by DBSP_SRC_FANOUT (validated away everywhere else).
+void run_rowfn(const dbsp_rowfn& f, const Env& e, u64* st, u64 j = 0) {
   int sp = 0;
   for (int pc = 0; pc < f.n_insn; pc++) {
     const dbsp_insn& in = f.code[pc];
@@ -19,7 +20,7 @@ void run_rowfn(const dbsp_rowfn& f, const Env& e, u64* st) {
       s.kind = in.kind;
       s.idx = in.idx;
       s.cst = in.cst;
-      st[sp++] = src_val(s, e);
+      st[sp++] = in.kind == DBSP_SRC_FANOUT ? j : src_val(s, e);
       continue;
     }
     const int pops = dbsp_validate::rowfn_arity(in.op);
@@ -66,9 +67,9 @@ void run_rowfn(const dbsp_rowfn& f, const Env& e, u64* st) {
   }
 }
 // the output row and whether the program keeps it
-bool project_fn(const dbsp_rowfn& f, const Env& e, u64* row) {
+bool project_fn(const dbsp_rowfn& f, const Env& e, u64* row, u64 j = 0) {
   u64 st[DBSP_MAX_STACK];
-  run_rowfn(f, e, st);
+  run_rowfn(f, e, st, j);
   const int nl = f.out_schema.n_key_lanes + f.out_schema.n_val_lanes;
   for (int l = 0; l < nl; l++) row[l] = st[l];
   return st[nl] != 0;
@@ -100,19 +101,29 @@ void join_into_fn(const Batch& L, const Batch& R, const dbsp_rowfn& f, bool swap
   }
 }
 
+// A fan-out of n rows into n * n_out rows before consolidation: the CUDA library's 32-bit bound, from the sizes.
+#define FANOUT_ROWS(n, n_out, what)                                                   \
+  do {                                                                                \
+    const std::string m__ = dv::valid_fanout_rows((n), (n_out), (what));              \
+    if (!m__.empty()) { g_err = m__; return DBSP_ERR_UNSUPPORTED; }                   \
+  } while (0)
+
+// n_out == 0: a plain row function (`_fn`); otherwise a fan-out whose program runs for j = 0 .. n_out-1 per row.
 int32_t table_to_batch_fn(const char* what, const u64* const* cols, uint32_t ncols, unsigned col_mask, const i64* w, u64 n,
-                          const dbsp_rowfn* fn, orc_batch** out) {
-  REFUSE(dv::valid_rowfn(fn, (int)ncols, (int)ncols, (int)ncols, what));
+                          const dbsp_rowfn* fn, orc_batch** out, uint32_t n_out = 0) {
+  REFUSE(dv::valid_rowfn(fn, (int)ncols, (int)ncols, (int)ncols, what, n_out != 0));
   const unsigned used = dv::rowfn_table_mask(*fn);
   CHECK_ARG((used & ~col_mask) == 0, std::string(what) + ": fn reads column " + std::to_string(__builtin_ctz((used & ~col_mask) | 0x100u)) +
                                          ", which col_mask left out of the upload");
   REFUSE(valid_cols(what, cols, (int)ncols, n, used));
+  FANOUT_ROWS(n, n_out, what);
   Tuples t(fn->out_schema);
   u64 lv[MAXL] = {0}, row[MAXL];
   for (u64 i = 0; i < n; i++) {
     for (uint32_t c = 0; c < ncols; c++) if ((used >> c) & 1) lv[c] = cols[c][i];
     Env e{lv, lv, lv};
-    if (project_fn(*fn, e, row)) t.push(row, w ? w[i] : 1);
+    for (u64 j = 0; j < std::max<u64>(n_out, 1); j++)
+      if (project_fn(*fn, e, row, j)) t.push(row, w ? w[i] : 1);
   }
   *out = wrap(t.build());
   return DBSP_OK;
@@ -145,6 +156,30 @@ int32_t orc_batch_from_upload_fn(orc_ctx* c, orc_upload* u, const dbsp_rowfn* fn
 
 uint32_t orc_rowfn_table_mask(const dbsp_rowfn* fn) {
   if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "rowfn_table_mask").empty()) return 0;
+  return dv::rowfn_table_mask(*fn);
+}
+
+// flat_map_index over a raw table with a fan-out (filter_map.rs:124-160: the closure returns an iterator).
+int32_t orc_batch_from_table_fanout(orc_ctx* c, const u64* const* cols, uint32_t ncols, const i64* w, u64 n, int32_t,
+                                    const dbsp_rowfn* fn, uint32_t n_out, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  CHECK_ARG(ncols >= 1 && ncols <= MAXL, "batch_from_table_fanout: n_cols = " + std::to_string(ncols) + ": a table has 1..8 columns");
+  REFUSE(dv::valid_fanout(n_out, WHAT));
+  ROWS32(n);
+  return table_to_batch_fn(WHAT, cols, ncols, ~0u, w, n, fn, out, n_out);
+}
+
+int32_t orc_batch_from_upload_fanout(orc_ctx* c, orc_upload* u, const dbsp_rowfn* fn, uint32_t n_out, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(u, "upload");
+  REFUSE(dv::valid_fanout(n_out, WHAT));
+  return table_to_batch_fn(WHAT, u->cols, u->n_cols, u->col_mask, u->w, u->n, fn, out, n_out);
+}
+
+uint32_t orc_fanout_table_mask(const dbsp_rowfn* fn) {
+  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "fanout_table_mask", true).empty()) return 0;
   return dv::rowfn_table_mask(*fn);
 }
 
@@ -214,13 +249,11 @@ int32_t orc_weigh_fn(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* f, int32_
   return DBSP_OK;
 }
 
-// Map/FlatMap/Index::eval + from_tuples (operator/filter_map.rs:563-577,700-724).
-int32_t orc_map_index_fn(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* fn, orc_batch** out) {
-  NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
+// Map/FlatMap/Index::eval + from_tuples (operator/filter_map.rs:563-577,700-724); n_out == 0: no fan-out.
+static int32_t map_index_fn(const char* what, const orc_batch* b, const dbsp_rowfn* fn, uint32_t n_out, orc_batch** out) {
   const Batch& B = *b->p;
-  REFUSE(dv::valid_rowfn(fn, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, WHAT));
+  REFUSE(dv::valid_rowfn(fn, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, what, n_out != 0));
+  FANOUT_ROWS(B.indexed() ? B.V.n : B.K.n, n_out, what);
   Tuples t(fn->out_schema);
   u64 key[MAXL], val[MAXL] = {0}, row[MAXL];
   for (size_t k = 0; k < B.K.n; k++) {
@@ -230,11 +263,28 @@ int32_t orc_map_index_fn(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* fn, o
     for (size_t v = lo; v < hi; v++) {
       if (B.indexed()) B.V.get(v, val);
       Env e{key, val, val};
-      if (project_fn(*fn, e, row)) t.push(row, B.w[v]);
+      for (u64 j = 0; j < std::max<u64>(n_out, 1); j++)
+        if (project_fn(*fn, e, row, j)) t.push(row, B.w[v]);
     }
   }
   *out = wrap(t.build());
   return DBSP_OK;
+}
+
+int32_t orc_map_index_fn(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* fn, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  return map_index_fn(WHAT, b, fn, 0, out);
+}
+
+// flat_map / flat_map_index of a batch with a fan-out: j = 0 .. n_out-1 per row, in one pass.
+int32_t orc_map_index_fanout(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* fn, uint32_t n_out, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(b, "batch");
+  REFUSE(dv::valid_fanout(n_out, WHAT));
+  return map_index_fn(WHAT, b, fn, n_out, out);
 }
 
 }  // extern "C"

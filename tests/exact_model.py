@@ -322,6 +322,41 @@ def flips(schema):
     return [SIGN if t == "i" else np.uint64(0) for t in schema.lanes]
 
 
+def lex_order(keyed):
+    """np.lexsort(keyed[::-1]) (stable, lane 0 most significant) for uint64 lanes, by np.sort alone: every lane's
+    offset from its minimum takes its bit width, the lanes are concatenated (the last lane least significant) and
+    the concatenation is sorted in digits of 64 - ib bits, least significant digit first, each digit with the
+    row's current position in the low ib bits (distinct words: np.sort is then a stable sort by the digit).
+    Returns (order, the digits of every pass in that order: equal rows have equal digits)."""
+    n = len(keyed[0])
+    ib = max((n - 1).bit_length(), 1)
+    dbits = 64 - ib
+    offs, bits = [], []
+    for c in keyed:
+        mn = c.min()
+        offs.append(c - mn)
+        bits.append(int(c.max() - mn).bit_length())
+    total, pos, at = sum(bits), [0] * len(keyed), 0
+    for l in range(len(keyed) - 1, -1, -1):
+        pos[l], at = at, at + bits[l]
+    low, sh = np.uint64((1 << ib) - 1), np.uint64(ib)
+    order, digits = None, []
+    for lo in range(0, max(total, 1), dbits):
+        hi = min(lo + dbits, total)
+        d = np.zeros(n, np.uint64)
+        for o, p, b in zip(offs, pos, bits):   # bits [lo, hi) of the concatenation
+            if b and p < hi and p + b > lo:
+                d |= (o >> np.uint64(max(lo - p, 0))) << np.uint64(max(p - lo, 0))
+        if hi > lo:
+            d &= np.uint64((1 << (hi - lo)) - 1)
+        s = np.sort(((d if order is None else d[order]) << sh) | np.arange(n, dtype=np.uint64))
+        perm = (s & low).astype(np.int64)
+        order = perm if order is None else order[perm]
+        digits.append(d)
+    # the last pass's digit comes out of the sort in order; the earlier ones are gathered
+    return order, [d[order] for d in digits[:-1]] + [s >> sh]
+
+
 def consolidate_np(schema, cols, weights):
     """from_tuples on numpy uint64 columns: sort by the typed lanes, sum equal rows mod 2^64, drop zero sums.
     Returns (sorted cols, weights)."""
@@ -330,20 +365,17 @@ def consolidate_np(schema, cols, weights):
         return [np.zeros(0, np.uint64) for _ in range(schema.nl)], np.zeros(0, np.int64)
     cols = [np.asarray(c).view(np.uint64) for c in cols]
     keyed = [c ^ f for c, f in zip(cols, flips(schema))]
-    order = np.lexsort(keyed[::-1]) if keyed else np.arange(n)
-    sc = [c[order] for c in cols]
+    order, digits = lex_order(keyed) if keyed else (np.arange(n), [])
     w = np.asarray(weights).view(np.uint64)[order]
     head = np.ones(n, bool)
-    if sc:
-        head[1:] = False
-        for c in sc:
-            head[1:] |= c[1:] != c[:-1]
-    else:
-        head[1:] = False
+    head[1:] = False
+    for d in digits:   # the packing is injective: rows differ iff some digit differs
+        head[1:] |= d[1:] != d[:-1]
     starts = np.flatnonzero(head)
     sums = np.add.reduceat(w, starts)   # uint64: wraps mod 2^64 by definition
     keep = sums != 0
-    return [c[starts][keep] for c in sc], sums[keep].view(np.int64)
+    rows = order[starts[keep]]
+    return [c[rows] for c in cols], sums[keep].view(np.int64)
 
 
 def canon(schema, cols, weights):

@@ -4,6 +4,7 @@ LSD fallback after the skew flag, multi-word keys."""
 import numpy as np
 import pytest
 
+import sort_plan_cases as sp
 from dbsp_b200 import Schema
 from parity_util import assert_batches_equal
 
@@ -26,16 +27,23 @@ def test_sort_sizes_and_widths(cuda, oracle, n, bits):
 
 @pytest.mark.parametrize("n", [50_000, 2_000_000])
 def test_sort_skew_falls_back(cuda, oracle, n):
-    """One hot key holds most rows: its bucket cannot fit a chunk, the LSD fallback must take over."""
+    """One hot key holds 70 % of the rows.  Below 256 K rows its top-digit bucket cannot fit a chunk and the LSD
+    fallback takes over; at 2 M rows the hot rows still differ in their 33-bit value lane, so the splitters divide
+    them and no bucket overflows.  A single key with random values sorts without a fallback, and rows that are all
+    equal arrive ordered and are not sorted at all.  The profile shows which plan each ran."""
+    hot_plan, single_plan = {50_000: ("top digit -> lsd fallback", "top digit"), 2_000_000: ("splitters(4096)",) * 2}[n]
     rng = np.random.default_rng(n)
     s = Schema("u", "u")
     k = np.where(rng.random(n) < 0.7, 12345, rng.integers(0, 1 << 30, n)).astype(np.uint64)
     v = rng.integers(0, 1 << 33, n).astype(np.uint64)
-    check(cuda, oracle, s, [k, v], rng.integers(-1, 2, n), "hot key")
-    # every key equal, values random
-    check(cuda, oracle, s, [np.full(n, 7, np.uint64), v], np.ones(n, np.int64), "single key")
-    # everything equal: one output row
-    check(cuda, oracle, s, [np.full(n, 7, np.uint64), np.full(n, 9, np.uint64)], np.ones(n, np.int64), "single row")
+    for what, cols, w, plan in [("hot key", [k, v], rng.integers(-1, 2, n), hot_plan),
+                                ("single key", [np.full(n, 7, np.uint64), v], np.ones(n, np.int64), single_plan),
+                                ("single row", [np.full(n, 7, np.uint64), np.full(n, 9, np.uint64)], np.ones(n, np.int64), "ordered")]:
+        cuda.profile(True)
+        check(cuda, oracle, s, cols, w, what)
+        prof = cuda.profile_read()
+        cuda.profile(False)
+        sp.check_plan(prof, n, sp.KeyPlan(s, cols, w), plan, what)
 
 
 @pytest.mark.parametrize("run", [1, 9, 900, 3000, 3073, 20_000])

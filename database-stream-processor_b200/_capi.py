@@ -137,6 +137,7 @@ _SIGS = {
     "weigh": [_P, _P, C.POINTER(CExpr), C.c_int32, _PP],
     "weigh_fn": [_P, _P, C.POINTER(CRowFn), C.c_int32, _PP],
     "distinct_delta": [_P, _P, _P, _PP],
+    "antijoin_delta": [_P, _P, _P, _P, _P, _PP],
     "stream_distinct": [_P, _P, _PP],
     "window_delta": [_P, _P, _P, C.c_int32, _U64P, _U64P, _U64P, _U64P, _PP],
     "map_index": [_P, _P, C.POINTER(CProj), _PP],
@@ -158,6 +159,9 @@ COMM_BLOB_BYTES = 128
 # them.  A library without them binds every other call, and calling one of them raises DbspError.
 ROWFN_CALLS = {"batch_from_table_fn", "batch_from_upload_fn", "join_delta_trace_fn", "join_batches_fn", "weigh_fn",
                "map_index_fn", "batch_from_table_fanout", "batch_from_upload_fanout", "map_index_fanout"}
+# Operators added after that oracle: the CUDA library and the row-function oracle export them, the dbsp_proj oracle
+# does not.  `CApi.exports` tells a caller which of them a library has.
+LATER_CALLS = {"antijoin_delta"}
 
 
 class CApi:
@@ -166,9 +170,11 @@ class CApi:
     def __init__(self, lib: C.CDLL, prefix: str):
         self.lib = lib
         self.prefix = prefix
+        self.missing = set()
         for name, argtypes in _SIGS.items():
-            if name in ROWFN_CALLS and not hasattr(lib, prefix + name):
-                setattr(self, "_" + name, self._not_exported(prefix + name))
+            if name in ROWFN_CALLS | LATER_CALLS and not hasattr(lib, prefix + name):
+                self.missing.add(name)
+                setattr(self, "_" + name, self._not_exported(prefix + name, name in ROWFN_CALLS))
                 continue
             fn = getattr(lib, prefix + name)  # AttributeError if a symbol is missing
             fn.argtypes = argtypes
@@ -192,10 +198,13 @@ class CApi:
                 fn = self._not_exported(prefix + mask)
             setattr(self, "_" + mask, fn)
 
+    def exports(self, name: str) -> bool:
+        return name not in self.missing
+
     @staticmethod
-    def _not_exported(symbol):
+    def _not_exported(symbol, rowfn=True):
         def refuse(*_):
-            raise DbspError(f"{symbol}: this library has no row functions")
+            raise DbspError(f"{symbol}: this library has no row functions" if rowfn else f"{symbol}: this library does not export it")
         return refuse
 
     @staticmethod

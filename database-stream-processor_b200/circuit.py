@@ -18,7 +18,7 @@ from typing import Callable, Sequence
 import numpy as np
 
 from . import _capi as capi
-from .zset import Backend, Batch, Proj, Schema, Spine, key, lval, rval
+from .zset import Backend, Batch, Expr, Fn, Pred, Proj, Schema, Spine, Src, const, key, lval, rval
 
 
 class Max:  # operator/aggregate/max.rs:36-55
@@ -35,6 +35,33 @@ class FoldCount:  # Fold counting distinct values (aggregate/mod.rs:908-916)
 
 class FoldSum:  # Fold summing distinct values (aggregate/mod.rs:918-929)
     kind = capi.AGG_FOLD_SUM
+
+
+class _KeyCounts:
+    """N(k), the number of distinct (k, v) rows of a stream's integral, as a trace of OrdZSet<K> counts.  step()
+    returns the change of the counts: distinct_delta's ±1 rows with their values dropped, which consolidation sums
+    per key."""
+
+    def __init__(self, be: Backend, schema: Schema):
+        self.be = be
+        self.keys = Proj(Schema(schema.key), [key(i) for i in range(schema.nk)])
+        self.trace = Spine(be, Schema(schema.key))
+
+    def step(self, delta: Batch, delayed_integral: Spine) -> Batch:
+        dn = self.be.map_index(self.be.distinct_delta(delta, delayed_integral), self.keys)
+        self.trace.insert(dn)
+        return dn
+
+
+def _zero_src(x, kind):
+    """The expression tree `x` with every source of `kind` read as 0."""
+    if isinstance(x, Src):
+        return const(0) if x.kind == kind else x
+    if isinstance(x, Expr):
+        return Expr(x.op, _zero_src(x.a, kind), _zero_src(x.b, kind))
+    if isinstance(x, Pred):
+        return Pred(x.cmp, _zero_src(x.a, kind), _zero_src(x.b, kind), x.is_signed)
+    return Fn(x.op, *[_zero_src(a, kind) for a in x.args])
 
 
 class Node:
@@ -310,7 +337,32 @@ class Stream:
     def antijoin(self, other: "Stream") -> "Stream":
         """antijoin (operator/join.rs:294-320): the rows of `self` whose key is
         absent from `other` = self - self |x| distinct(other) with the identity
-        closure (k, v1)."""
+        closure (k, v1).  A row (k, v1, w) gets the weight w·(1 − N(k)), N(k)
+        being the number of distinct (k, v2) rows of `other`; so a key with two
+        or more of them gives negative weights, as in the reference.
+
+        Keyed streams keep N as a trace of per-key counts and run
+        dbsp_antijoin_delta, which never expands a key's values against the
+        other side's.  A key-less stream runs the composition above."""
+        be = self.circuit.be
+        if self.schema.nk == 0 or not be.api.exports("antijoin_delta"):
+            return self._antijoin_composed(other)
+        left, right = self.shard_with(other)
+        a, ib = Spine(be, left.schema), Spine(be, right.schema)   # z^-1 of self's and other's integrals
+        nb = _KeyCounts(be, right.schema)
+
+        def fn(da: Batch, db: Batch):
+            dnb = nb.step(db, ib)
+            ib.insert(db)
+            out = be.antijoin_delta(da, a, dnb, nb.trace)
+            a.insert(da)
+            return out
+
+        return left._binary(right, fn, "antijoin", self.schema, True)   # mark_sharded (join.rs:316)
+
+    def _antijoin_composed(self, other: "Stream") -> "Stream":
+        """self - self |x| distinct(other), as join.rs:294-320 composes it: the only antijoin of a key-less stream
+        (the join is then a cross product), and the one of a library without dbsp_antijoin_delta."""
         s1 = self.shard()
         s2 = other.distinct().shard()
         nk, nv = self.schema.nk, self.schema.nv
@@ -318,6 +370,47 @@ class Stream:
         out = s1.minus(s1.join(s2, ident))
         out.sharded = True   # mark_sharded (join.rs:316)
         return out
+
+    def outer_join(self, other: "Stream", f: Proj, fl: Proj, fr: Proj) -> "Stream":
+        """outer_join (operator/join.rs:332-360) = join(f) + antijoin(self, other).map(fl) + antijoin(other, self)
+        .map(fr): SQL's FULL OUTER JOIN.  `f` is a join closure (key / lval / rval), `fl` a map closure over self's
+        rows, `fr` one over other's rows (their values are lval, and rval reads the same lanes); all three have one
+        out_schema.  The join's two traces are also the antijoins' traces and the delayed integrals their key
+        counts come from, so each input is held once."""
+        for name, p in (("f", f), ("fl", fl), ("fr", fr)):
+            if p.is_fanout:
+                raise ValueError(f"outer_join: {name} is a fan-out closure; an outer join yields one row per match or row")
+        if fl.schema != f.schema or fr.schema != f.schema:
+            raise ValueError(f"outer_join: f, fl and fr must have one out_schema, have {f.schema}, {fl.schema}, {fr.schema}")
+        if self.schema.nk == 0:
+            raise ValueError("outer_join: a key-less stream has no key set to count")
+        be = self.circuit.be
+        left, right = self.shard_with(other)
+        lt, rt = Spine(be, left.schema), Spine(be, right.schema)
+        na, nb = _KeyCounts(be, left.schema), _KeyCounts(be, right.schema)
+
+        def fn(dl: Batch, dr: Batch):
+            # every read sees the state the formula names: the counts and antijoins use z^-1 of the integrals
+            dna, dnb = na.step(dl, lt), nb.step(dr, rt)
+            ol = be.map_index(be.antijoin_delta(dl, lt, dnb, nb.trace), fl)
+            orr = be.map_index(be.antijoin_delta(dr, rt, dna, na.trace), fr)
+            rt.insert(dr)                                             # then Stream.join's order
+            o1 = be.join_delta_trace(dl, rt, f, delta_is_left=True)
+            o2 = be.join_delta_trace(dr, lt, f, delta_is_left=False)
+            lt.insert(dl)
+            return be.merge(be.merge(o1, o2), be.merge(ol, orr))
+
+        return left._binary(right, fn, "outer_join", f.schema)
+
+    def outer_join_default(self, other: "Stream", f: Proj) -> "Stream":
+        """outer_join_default (operator/join.rs:362-386): outer_join with fl = f over a right value of zeros and
+        fr = f over a left value of zeros (Default::default() of u64 / i64).  A filter of `f` (its `where`) is part
+        of the closure: it holds or not for the matched rows as it does in join(f), and for an unmatched row it is
+        evaluated with the missing side's value lanes read as 0, like the output lanes.  The reference's closure has
+        no separate filter, so with one this goes beyond it."""
+        fl = Proj(f.schema, [_zero_src(o, capi.SRC_RVAL) for o in f.out], [_zero_src(w, capi.SRC_RVAL) for w in f.where])
+        fr = Proj(f.schema, [_zero_src(o, capi.SRC_LVAL) for o in f.out], [_zero_src(w, capi.SRC_LVAL) for w in f.where])
+        return self.outer_join(other, f, fl, fr)
 
     def join_incremental(self, other: "Stream", proj: Proj) -> "Stream":
         """join_incremental (operator/join.rs:136-155):

@@ -1411,6 +1411,15 @@ int32_t dbsp_distinct_delta(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine
   NOT_NULL(i, "delayed_integral");
   CHECK_ARG(dv::same_schema(B(d)->s, i->s), "distinct_delta: delta and delayed_integral differ in schema");
   OUT1(op_distinct_delta(ctx, B(d), i, &o__)) }
+int32_t dbsp_antijoin_delta(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* t, const dbsp_batch* kd,
+                            const dbsp_spine* kt, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(d, "delta");
+  NOT_NULL(t, "trace");
+  NOT_NULL(kd, "key_delta");
+  NOT_NULL(kt, "key_trace");
+  REFUSE(dv::valid_antijoin(B(d)->s, t->s, B(kd)->s, kt->s));
+  OUT1(op_antijoin_delta(ctx, B(d), t, B(kd), kt, &o__)) }
 int32_t dbsp_stream_distinct(dbsp_ctx* ctx, const dbsp_batch* b, dbsp_batch** out) { ENTER(ctx);
   NOT_NULL(out, "out");
   NOT_NULL(b, "batch");

@@ -579,6 +579,17 @@ __global__ void k_distinct_decide(const i64* wD, const i64* oldw, u64 n, u32* ke
   neww[i] = w;
 }
 
+// The antijoin's weight of a delta row whose key has acc distinct values on the other side: w·(1 − acc), wrapping
+// (join.rs:294-320: self − self ⋈ distinct(other)).  A row whose weight is 0 is dropped.
+__global__ void k_antijoin_scale(const i64* wD, const i64* acc, u64 n, u32* keep, i64* neww) {
+  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > n) return;
+  if (i == n) { keep[n] = 0; return; }
+  const i64 w = (i64)((u64)wD[i] * ((u64)1 - (u64)acc[i]));
+  keep[i] = w != 0;
+  neww[i] = w;
+}
+
 // IndexedZSet::distinct (algebra/zset/mod.rs:14-38).
 __global__ void k_positive(const i64* w, u64 n, u32* keep, i64* neww) {
   u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1396,6 +1407,60 @@ int32_t op_distinct_delta(Ctx* ctx, const Batch* delta, const Spine* integral, B
   k_distinct_decide<<<blocks(n + 1), TB, 0, st>>>(delta->w, acc, n, (u32*)kb->p, neww);
   LAUNCH_COUNT(ctx);
   return compact_ordered(ctx, delta->s, delta->cols(), neww, (u32*)kb->p, n, out);
+}
+
+// antijoin (operator/join.rs:294-320) incrementally, with N(k) the count of k's distinct values on the other side:
+// out = delta·(1 − N_t) − trace ⋉ ΔN.  The first term is one lookup per delta row and keeps delta's order, so it
+// needs no sort; the second gathers only the trace rows of the keys whose count changed.  Neither expands a key's
+// values against the other side's.
+int32_t op_antijoin_delta(Ctx* ctx, const Batch* delta, const Spine* trace, const Batch* key_delta,
+                          const Spine* key_trace, Batch** out) {
+  const int nk = delta->s.n_key_lanes, nv = delta->s.n_val_lanes;
+  const u64 n = delta->n;
+  Batch* first = nullptr;
+  if (n == 0) {
+    first = batch_new_empty(ctx, delta->s);
+  } else {
+    cudaStream_t st = ctx->stream;
+    BufP ab, kb;
+    TRY(dev_alloc(ctx, (size_t)n * 8 * 2, &ab));
+    TRY(dev_alloc(ctx, (size_t)(n + 1) * 4, &kb));
+    i64* acc = (i64*)ab->p;
+    i64* neww = acc + n;
+    CUDA_TRY(cudaMemsetAsync(acc, 0, (size_t)n * 8, st));
+    for (Batch* T : key_trace->batches) {
+      k_lookup_add<<<blocks(n), TB, 0, st>>>(delta->cols(), n, T->cols(), T->w, T->n, nk, delta->flips(), acc);
+      LAUNCH_COUNT(ctx);
+    }
+    {
+      ProfScope ps(ctx, KID_ANTIJOIN, n * (8 + 8 + 8 + 4));   // weights and counts read, weights and flags written
+      k_antijoin_scale<<<blocks(n + 1), TB, 0, st>>>(delta->w, acc, n, (u32*)kb->p, neww);
+    }
+    LAUNCH_COUNT(ctx);
+    TRY(compact_ordered(ctx, delta->s, delta->cols(), neww, (u32*)kb->p, n, &first));
+  }
+  // the identity closure (k, v1) over the trace's rows: weight Δcount · w_trace
+  dbsp_proj ident;
+  memset(&ident, 0, sizeof(ident));
+  ident.out_schema = delta->s;
+  for (int l = 0; l < nk + nv; l++) {
+    ident.out[l].op = DBSP_OP_COPY;
+    ident.out[l].a.kind = l < nk ? DBSP_SRC_KEY : DBSP_SRC_LVAL;
+    ident.out[l].a.idx = (uint8_t)(l < nk ? l : l - nk);
+  }
+  Batch* gathered = nullptr;
+  int32_t rc = probe_spine(ctx, key_delta, nk, trace, &ident, 0, delta->s, &gathered);
+  if (rc != DBSP_OK) { batch_unref(first); return rc; }
+  if (gathered->n == 0) { batch_unref(gathered); *out = first; return DBSP_OK; }
+  Batch* neg = nullptr;
+  rc = op_neg(ctx, gathered, &neg);
+  batch_unref(gathered);
+  if (rc == DBSP_OK) {
+    rc = merge_batches(ctx, first, neg, out);
+    batch_unref(neg);
+  }
+  batch_unref(first);
+  return rc;
 }
 
 // IndexedZSet::distinct (algebra/zset/mod.rs:14-38)

@@ -29,6 +29,8 @@ int32_t op_neg(Ctx* ctx, const Batch* a, Batch** out);
 template <class F>
 int32_t op_weigh(Ctx* ctx, const Batch* b, const F* f, int mode, Batch** out);
 int32_t op_distinct_delta(Ctx* ctx, const Batch* delta, const Spine* integral, Batch** out);
+int32_t op_antijoin_delta(Ctx* ctx, const Batch* delta, const Spine* trace, const Batch* key_delta,
+                          const Spine* key_trace, Batch** out);
 int32_t op_stream_distinct(Ctx* ctx, const Batch* b, Batch** out);
 int32_t op_semijoin(Ctx* ctx, const Batch* pairs, const Batch* keys, Batch** out);
 int32_t op_window_delta(Ctx* ctx, const Spine* trace, const Batch* delta, int has_prev, const u64* s0, const u64* e0,

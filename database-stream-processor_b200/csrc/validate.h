@@ -172,6 +172,20 @@ inline std::string valid_aggregate(const dbsp_schema& delta, const dbsp_schema& 
   return "";
 }
 
+// antijoin_delta: delta and trace share one schema with at least one key lane (a key-less stream has no key set to
+// count); key_delta and key_trace have exactly delta's key lanes and no value lanes.
+inline std::string valid_antijoin(const dbsp_schema& delta, const dbsp_schema& trace, const dbsp_schema& key_delta,
+                                  const dbsp_schema& key_trace) {
+  const std::string what = "antijoin_delta";
+  if (!same_schema(delta, trace)) return what + ": delta and trace differ in schema";
+  if (delta.n_key_lanes == 0) return what + ": delta has no key lanes, so there is no key set to count";
+  if (!same_key_lanes(delta, key_delta) || key_delta.n_val_lanes != 0)
+    return what + ": key_delta must have exactly delta's key lanes (count and type) and no value lanes";
+  if (!same_key_lanes(delta, key_trace) || key_trace.n_val_lanes != 0)
+    return what + ": key_trace must have exactly delta's key lanes (count and type) and no value lanes";
+  return "";
+}
+
 // ---- snapshot files (dbsp_spine_save / dbsp_spine_load) ---------------------------------------------------------
 // header: magic, schema, {has key bound, has value bound, effort, layer count}, key bound, value bound
 inline std::string valid_snapshot_header(const dbsp_schema& s, const uint64_t hdr[4]) {

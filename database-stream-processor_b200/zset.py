@@ -938,6 +938,13 @@ class Backend:
         self.api.call("distinct_delta", self.ctx, delta.h, integral.h, C.byref(out))
         return Batch(self, out.value, delta.schema)
 
+    def antijoin_delta(self, delta: Batch, trace: Spine, key_delta: Batch, key_trace: Spine) -> Batch:
+        """delta·(1 − key_trace(k)) − trace ⋉ key_delta: the antijoin's change, with the keys' distinct-value counts
+        (OrdZSet<K>) in place of distinct(other)."""
+        out = self._out()
+        self.api.call("antijoin_delta", self.ctx, delta.h, trace.h, key_delta.h, key_trace.h, C.byref(out))
+        return Batch(self, out.value, delta.schema)
+
     def stream_distinct(self, b: Batch) -> Batch:
         out = self._out()
         self.api.call("stream_distinct", self.ctx, b.h, C.byref(out))

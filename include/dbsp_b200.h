@@ -471,6 +471,20 @@ int32_t dbsp_weigh_fn(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_rowfn* fn,
 int32_t dbsp_distinct_delta(dbsp_ctx* ctx, const dbsp_batch* delta,
                             const dbsp_spine* delayed_integral,
                             dbsp_batch** out);
+/* The change of antijoin (operator/join.rs:294-320) without expanding a key's
+ * values.  With N(k) the number of distinct (k, v2) rows of the other side
+ * (the rows of distinct(other) on key k), the antijoin gives a row (k, v1, w)
+ * the weight w·(1 − N(k)), wrapping; so its change is
+ *   out = delta·(1 − key_trace(k)) − trace ⋉ key_delta,
+ * consolidated, with delta's schema.  `trace` is z^-1 of delta's integral
+ * (delta's schema).  `key_delta` and `key_trace` are OrdZSet<K>s with exactly
+ * delta's key lanes (count and types) and no value lanes: a row's weight is
+ * the change of its key's count (key_delta) or the count itself (key_trace,
+ * which already includes key_delta; key_trace(k) sums k's weights over its
+ * batches).  delta has at least one key lane. */
+int32_t dbsp_antijoin_delta(dbsp_ctx* ctx, const dbsp_batch* delta,
+                            const dbsp_spine* trace, const dbsp_batch* key_delta,
+                            const dbsp_spine* key_trace, dbsp_batch** out);
 /* IndexedZSet::distinct (algebra/zset/mod.rs:14-38). */
 int32_t dbsp_stream_distinct(dbsp_ctx* ctx, const dbsp_batch* b,
                              dbsp_batch** out);

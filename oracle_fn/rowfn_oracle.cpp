@@ -1,8 +1,8 @@
 // rowfn_oracle.cpp — the CPU oracle with row functions (dbsp_rowfn, include/dbsp_b200.h): the whole oracle of
-// oracle/dbsp_oracle.cpp, unchanged, plus the `_fn` and `_fanout` entry points, in one translation unit so that they build on its
+// oracle/dbsp_oracle.cpp, unchanged, plus the `_fn` and `_fanout` entry points and dbsp_antijoin_delta, in one translation unit so that they build on its
 // batches, traces, consolidation and error text.  The oracle's own library stays the checker of every `dbsp_proj`
 // test; this one (libdbsp_oracle_fn.so, test infrastructure like it, never linked into the product) is the checker
-// of the row-function tests.  The interpreter below is written apart from the CUDA library's; validate.h is shared,
+// of the row-function and antijoin tests.  The interpreter below is written apart from the CUDA library's; validate.h is shared,
 // so both libraries refuse the same programs with the same texts.
 #include "../oracle/dbsp_oracle.cpp"
 
@@ -176,6 +176,53 @@ int32_t orc_batch_from_upload_fanout(orc_ctx* c, orc_upload* u, const dbsp_rowfn
   NOT_NULL(u, "upload");
   REFUSE(dv::valid_fanout(n_out, WHAT));
   return table_to_batch_fn(WHAT, u->cols, u->n_cols, u->col_mask, u->w, u->n, fn, out, n_out);
+}
+
+// antijoin (operator/join.rs:294-320) incrementally, as the formula reads: a delta row (k, v1, w) with N(k) distinct
+// values on the other side gets w·(1 − N(k)), and every trace row (k, v1, w') of a key whose count changed by dN
+// adds −dN·w'.  Written apart from the CUDA library's lookups and gather.
+int32_t orc_antijoin_delta(orc_ctx* c, const orc_batch* delta, const orc_spine* tr, const orc_batch* kd,
+                           const orc_spine* kt, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(delta, "delta");
+  NOT_NULL(tr, "trace");
+  NOT_NULL(kd, "key_delta");
+  NOT_NULL(kt, "key_trace");
+  REFUSE(dv::valid_antijoin(delta->p->s, tr->s.s, kd->p->s, kt->s.s));
+  const Batch& D = *delta->p;
+  const int nk = D.s.n_key_lanes;
+  Tuples t(D.s);
+  std::vector<std::pair<KV, i64>> grp;
+  u64 row[MAXL];
+  for (size_t k = 0; k < D.K.n; k++) {
+    D.K.get(k, row);
+    key_group(kt->s, row, grp);   // no value lanes: one group, the key's count summed over the batches
+    const u64 one_minus_n = (u64)1 - (u64)(grp.empty() ? 0 : grp[0].second);
+    size_t lo, hi;
+    D.vrange(k, lo, hi);
+    for (size_t v = lo; v < hi; v++) {
+      if (D.indexed()) D.V.get(v, row + nk);
+      t.push(row, (i64)((u64)D.w[v] * one_minus_n));
+    }
+  }
+  const Batch& KD = *kd->p;
+  for (size_t k = 0; k < KD.K.n; k++) {
+    KD.K.get(k, row);
+    for (auto& bp : tr->s.batches) {
+      const Batch& b = *bp;
+      const size_t i = seek_key(b, 0, row);
+      if (i >= b.K.n || cmp_row_tuple(b.K, i, row) != 0) continue;
+      size_t lo, hi;
+      b.vrange(i, lo, hi);
+      for (size_t v = lo; v < hi; v++) {
+        if (b.indexed()) b.V.get(v, row + nk);
+        t.push(row, (i64)((u64)0 - (u64)KD.w[k] * (u64)b.w[v]));
+      }
+    }
+  }
+  *out = wrap(t.build());
+  return DBSP_OK;
 }
 
 uint32_t orc_fanout_table_mask(const dbsp_rowfn* fn) {

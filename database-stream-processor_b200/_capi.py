@@ -15,12 +15,13 @@ MAX_PREDS = 4
 MAX_INSNS = 64
 MAX_STACK = 16
 MAX_FANOUT = 64
+MAX_ACC = 15
 
 OK = 0
 ERR_NAMES = {1: "DBSP_ERR_INVALID", 2: "DBSP_ERR_CUDA", 3: "DBSP_ERR_NO_DEVICE", 4: "DBSP_ERR_UNSUPPORTED"}
 
 U64, I64 = 0, 1
-SRC_KEY, SRC_LVAL, SRC_RVAL, SRC_CONST, SRC_FANOUT = 0, 1, 2, 3, 4
+SRC_KEY, SRC_LVAL, SRC_RVAL, SRC_CONST, SRC_FANOUT, SRC_ACC, SRC_WEIGHT = 0, 1, 2, 3, 4, 5, 6
 OP_COPY, OP_NEG, OP_ADD, OP_SUB, OP_MUL, OP_DIV = range(6)
 CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_IN = range(7)
 AGG_MAX, AGG_MIN, AGG_FOLD_COUNT, AGG_FOLD_SUM, AGG_WCOUNT, AGG_WCOUNT2 = range(6)
@@ -62,6 +63,11 @@ class CInsn(C.Structure):
 
 class CRowFn(C.Structure):
     _fields_ = [("out_schema", CSchema), ("n_insn", C.c_uint8), ("pad_", C.c_uint8 * 5), ("code", CInsn * MAX_INSNS)]
+
+
+class CFold(C.Structure):
+    _fields_ = [("n_acc", C.c_uint8), ("n_step", C.c_uint8), ("pad_", C.c_uint8 * 6), ("init", C.c_uint64 * MAX_ACC),
+                ("step", CInsn * MAX_INSNS), ("output", CRowFn)]
 
 
 class DbspError(RuntimeError):
@@ -134,6 +140,7 @@ _SIGS = {
     "join_batches_fn": [_P, _P, _P, C.POINTER(CRowFn), _PP],
     "semijoin": [_P, _P, _P, _PP],
     "aggregate_delta": [_P, _P, _P, _P, C.c_int32, _PP],
+    "aggregate_fold": [_P, _P, _P, _P, C.POINTER(CFold), _PP],
     "weigh": [_P, _P, C.POINTER(CExpr), C.c_int32, _PP],
     "weigh_fn": [_P, _P, C.POINTER(CRowFn), C.c_int32, _PP],
     "distinct_delta": [_P, _P, _P, _PP],
@@ -161,7 +168,7 @@ ROWFN_CALLS = {"batch_from_table_fn", "batch_from_upload_fn", "join_delta_trace_
                "map_index_fn", "batch_from_table_fanout", "batch_from_upload_fanout", "map_index_fanout"}
 # Operators added after that oracle: the CUDA library and the row-function oracle export them, the dbsp_proj oracle
 # does not.  `CApi.exports` tells a caller which of them a library has.
-LATER_CALLS = {"antijoin_delta"}
+LATER_CALLS = {"antijoin_delta", "aggregate_fold"}
 
 
 class CApi:

@@ -18,7 +18,8 @@ from typing import Callable, Sequence
 import numpy as np
 
 from . import _capi as capi
-from .zset import Backend, Batch, Expr, Fn, Pred, Proj, Schema, Spine, Src, const, key, lval, rval
+from .zset import (Backend, Batch, Expr, Fn, Pred, Proj, Schema, Spine, Src, acc, compile_fold, compile_fold_step, const, key,
+                   lval, rval)
 
 
 class Max:  # operator/aggregate/max.rs:36-55
@@ -35,6 +36,34 @@ class FoldCount:  # Fold counting distinct values (aggregate/mod.rs:908-916)
 
 class FoldSum:  # Fold summing distinct values (aggregate/mod.rs:918-929)
     kind = capi.AGG_FOLD_SUM
+
+
+class Fold:
+    """Fold::new / Fold::with_output (operator/aggregate/fold.rs), the general aggregator: per key, `init`, then
+    `step` applied in value order to each value whose weight (summed over the trace) is non-zero, then `output`.
+
+    init: the accumulator's n_acc (1..15) words.  step: n_acc expressions, the new words, over key(i), lval(i) / val(i)
+    (the value's lanes), acc(i), weight() and constants.  where: the step's keep condition(s); a value for which it
+    does not hold leaves the accumulator unchanged.  output: a Proj over key(i) / acc(i) with value lanes only (its
+    filter drops the key's row); by default the accumulator itself, typed u (n_acc <= 8).  A key with no value of
+    non-zero weight has no row.  Fold is not a semigroup (UnimplementedSemigroup): every key is walked serially."""
+
+    def __init__(self, init: Sequence[int], step: Sequence, output: Proj | None = None, where=None):
+        init = [int(x) for x in init]
+        if len(step) != len(init):
+            raise ValueError(f"Fold: init has {len(init)} accumulator words and step gives {len(step)}")
+        where = [] if where is None else list(where) if isinstance(where, (list, tuple)) else [where]
+        code = compile_fold_step(step, where)
+        if output is None:
+            if len(init) > capi.MAX_LANES:
+                raise ValueError(f"Fold: an accumulator of {len(init)} words needs an output of at most {capi.MAX_LANES} lanes")
+            output = Proj(Schema("", "u" * len(init)), [acc(i) for i in range(len(init))])
+        if output.schema.nk != 0:
+            raise ValueError("Fold: the output has key lanes; it gives the key's value lanes only")
+        if output.is_fanout:
+            raise ValueError("Fold: the output is a fan-out closure; a key has one output")
+        self.init, self.step, self.where, self.output = init, list(step), where, output
+        self._c = compile_fold(init, code, output._c if output.is_fn else output.as_rowfn()._c)
 
 
 class _KeyCounts:
@@ -438,6 +467,11 @@ class Stream:
         (MinSemigroup / MaxSemigroup, aggregate/min.rs:17-27), whose partial
         results are then aggregated again after a shard of <= P rows per key."""
         be = self.circuit.be
+        if isinstance(aggregator, Fold):
+            if local:
+                raise ValueError("aggregate(Fold, local=True): Fold is not a semigroup, so per-worker partial folds "
+                                 "cannot be combined")
+            return self._aggregate_fold(aggregator)
         s = Stream(self.circuit, self.node, self.schema, True) if local else self.shard()
         kind = aggregator.kind
         if kind in (capi.AGG_MAX, capi.AGG_MIN):
@@ -454,6 +488,26 @@ class Stream:
 
         return s._unary(fn, "aggregate", out_schema, not local)
 
+    def _fold_schema(self, fold: Fold) -> Schema:
+        api = self.circuit.be.api
+        if not api.exports("aggregate_fold"):
+            raise capi.DbspError(f"{api.prefix}aggregate_fold: this library does not export it")
+        return Schema(self.schema.key, fold.output.schema.val)
+
+    def _aggregate_fold(self, fold: Fold) -> "Stream":
+        be = self.circuit.be
+        out_schema = self._fold_schema(fold)
+        s = self.shard()
+        in_tr, out_tr = Spine(be, s.schema), Spine(be, out_schema)
+
+        def fn(d: Batch):
+            in_tr.insert(d)
+            out = be.aggregate_fold(d, in_tr, out_tr, fold)
+            out_tr.insert(out)
+            return out
+
+        return s._unary(fn, "aggregate", out_schema, True)
+
     def stream_aggregate(self, aggregator) -> "Stream":
         """stream_aggregate (operator/aggregate/mod.rs:172-196): Aggregate::eval
         (:362-376) — the aggregate of every key of *this step's* batch with
@@ -461,15 +515,24 @@ class Stream:
         holding only the batch and an empty output trace."""
         be = self.circuit.be
         s = self.shard()
-        kind = aggregator.kind
-        out_schema = s.schema if kind in (capi.AGG_MAX, capi.AGG_MIN) else Schema(s.schema.key, "u")
+        if isinstance(aggregator, Fold):
+            out_schema = self._fold_schema(aggregator)
+
+            def run(d, tin, tout):
+                return be.aggregate_fold(d, tin, tout, aggregator)
+        else:
+            kind = aggregator.kind
+            out_schema = s.schema if kind in (capi.AGG_MAX, capi.AGG_MIN) else Schema(s.schema.key, "u")
+
+            def run(d, tin, tout):
+                return be.aggregate_delta(d, tin, tout, kind)
 
         def fn(d: Batch):
             if len(d) == 0:
                 return be.batch_empty(out_schema)
             tin, tout = Spine(be, s.schema), Spine(be, out_schema)
             tin.insert(d)
-            return be.aggregate_delta(d, tin, tout, kind)
+            return run(d, tin, tout)
 
         return s._unary(fn, "stream_aggregate", out_schema, True)
 

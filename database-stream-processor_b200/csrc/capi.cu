@@ -554,7 +554,7 @@ int32_t dbsp_batch_from_table_fanout(dbsp_ctx* ctx, const uint64_t* const* cols,
   NOT_NULL(out, "out");
   CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "batch_from_table_fanout: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
   REFUSE(dv::valid_fanout(n_out, WHAT));
-  REFUSE(dv::valid_rowfn(fn, (int)n_cols, (int)n_cols, (int)n_cols, WHAT, true));
+  REFUSE(dv::valid_rowfn(fn, (int)n_cols, (int)n_cols, (int)n_cols, WHAT, dv::SRC_BIT_FANOUT));
   REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, dv::rowfn_table_mask(*fn)));
   ROWS32(n);
   FANOUT_ROWS(n, n_out);
@@ -588,7 +588,7 @@ uint32_t dbsp_rowfn_table_mask(const dbsp_rowfn* fn) {
   return dv::rowfn_table_mask(*fn);
 }
 uint32_t dbsp_fanout_table_mask(const dbsp_rowfn* fn) {
-  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "fanout_table_mask", true).empty()) return 0;
+  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "fanout_table_mask", dv::SRC_BIT_FANOUT).empty()) return 0;
   return dv::rowfn_table_mask(*fn);
 }
 
@@ -684,7 +684,7 @@ int32_t dbsp_batch_from_upload_fanout(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_
   NOT_NULL(u, "upload");
   CHECK_ARG(u->ctx == ctx, "batch_from_upload_fanout: upload belongs to another context");
   REFUSE(dv::valid_fanout(n_out, WHAT));
-  REFUSE(dv::valid_rowfn(fn, u->n_cols, u->n_cols, u->n_cols, WHAT, true));
+  REFUSE(dv::valid_rowfn(fn, u->n_cols, u->n_cols, u->n_cols, WHAT, dv::SRC_BIT_FANOUT));
   {
     const unsigned missing = dv::rowfn_table_mask(*fn) & ~u->col_mask;
     CHECK_ARG(missing == 0, "batch_from_upload_fanout: fn reads column " + std::to_string(__builtin_ctz(missing | 0x100u)) + ", which col_mask left out of the upload");
@@ -1388,6 +1388,14 @@ int32_t dbsp_aggregate_delta(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spin
   NOT_NULL(out_tr, "out_trace");
   REFUSE(dv::valid_aggregate(B(d)->s, in_tr->s, out_tr->s, kind));
   OUT1(op_aggregate_delta(ctx, B(d), in_tr, out_tr, kind, &o__)) }
+int32_t dbsp_aggregate_fold(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* in_tr, const dbsp_spine* out_tr,
+                            const dbsp_fold* fold, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(d, "delta");
+  NOT_NULL(in_tr, "in_trace");
+  NOT_NULL(out_tr, "out_trace");
+  REFUSE(dv::valid_fold(B(d)->s, in_tr->s, out_tr->s, fold));
+  OUT1(op_aggregate_fold(ctx, B(d), in_tr, out_tr, fold, &o__)) }
 int32_t dbsp_weigh(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_expr* f, int32_t mode, dbsp_batch** out) { ENTER(ctx);
   NOT_NULL(out, "out");
   NOT_NULL(b, "batch");
@@ -1448,7 +1456,7 @@ int32_t dbsp_map_index_fanout(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_row
   NOT_NULL(out, "out");
   NOT_NULL(b, "batch");
   REFUSE(dv::valid_fanout(n_out, WHAT));
-  REFUSE(dv::valid_rowfn(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT, true));
+  REFUSE(dv::valid_rowfn(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT, dv::SRC_BIT_FANOUT));
   FANOUT_ROWS(B(b)->n, n_out);
   const RowFnFanout fo = fanout_of(*f, n_out);
   OUT1(op_map_index(ctx, B(b), &fo, &o__)) }

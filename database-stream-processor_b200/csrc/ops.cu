@@ -2,6 +2,7 @@
 // aggregate, distinct), window ranges, shard partition.  Each host entry
 // cites the reference `eval` it replaces (paths under crates/dbsp/src/).
 #include "ops.cuh"
+#include "validate.h"
 
 namespace {
 
@@ -43,6 +44,18 @@ struct FanEnv {
   int nk;
   u64 row;
   u64 j;
+  __device__ __forceinline__ u64 k(int i) const { return c.c[i][row]; }
+  __device__ __forceinline__ u64 l(int i) const { return c.c[nk + i][row]; }
+  __device__ __forceinline__ u64 r(int i) const { return c.c[nk + i][row]; }
+};
+// one step of a Fold (dbsp_fold): row `row` of a gathered key group, the accumulator and the row's summed weight
+// (DBSP_SRC_ACC / DBSP_SRC_WEIGHT); the output program runs in it too, reading only the key and the accumulator
+struct FoldEnv {
+  const Cols& c;
+  int nk;
+  u64 row;
+  const u64* acc;
+  i64 w;
   __device__ __forceinline__ u64 k(int i) const { return c.c[i][row]; }
   __device__ __forceinline__ u64 l(int i) const { return c.c[nk + i][row]; }
   __device__ __forceinline__ u64 r(int i) const { return c.c[nk + i][row]; }
@@ -118,6 +131,10 @@ __device__ __forceinline__ void run_rowfn(const dbsp_rowfn& f, const E& e, u64* 
         default:
           if constexpr (std::is_same<E, FanEnv>::value) {   // only a fan-out's environment has a j
             if (in.kind == DBSP_SRC_FANOUT) { v = e.j; break; }
+          }
+          if constexpr (std::is_same<E, FoldEnv>::value) {   // only a fold's environment has acc and a weight
+            if (in.kind == DBSP_SRC_ACC) { v = e.acc[in.idx]; break; }
+            if (in.kind == DBSP_SRC_WEIGHT) { v = (u64)e.w; break; }
           }
           v = (u64)in.cst;
       }
@@ -714,6 +731,45 @@ __global__ void k_agg_pick(Cols G, const i64* wG, u64 n, int nk, int nv, int kin
     for (int l = 0; l < out_nv; l++) out.c[l][i] = v[l];
 }
 
+// A Fold's two programs as kernel parameters: the step as a dbsp_rowfn (validate.h's fold_step_rowfn) so that
+// run_rowfn runs both, and the accumulator's first value.
+struct FoldArgs {
+  dbsp_rowfn step;
+  dbsp_rowfn output;
+  u64 init[DBSP_MAX_ACC];
+  int n_acc;
+};
+// Fold (fold.rs:60-75) over a gathered, consolidated key group batch G (the affected keys' rows in value order,
+// weights summed over the spine's batches, zeros dropped).  Fold is not associative, so a key is walked serially: the
+// thread of the key's first row runs `step` on each of the key's rows in order, then `output`, and writes the output
+// lanes and the keep flag at that row.  Every other row gets keep = 0.  Every row of G has a non-zero weight, so every
+// key in G is non-empty.
+__global__ void k_agg_fold(Cols G, const i64* wG, u64 n, int nk, FoldArgs fa, u32* keep, MCols out, int out_nv) {
+  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > n) return;
+  if (i == n) { keep[n] = 0; return; }
+  bool first = i == 0;
+  if (!first)
+    for (int l = 0; l < nk; l++)
+      if (G.c[l][i] != G.c[l][i - 1]) { first = true; break; }
+  if (!first) { keep[i] = 0; return; }
+  u64 acc[DBSP_MAX_ACC];
+  for (int a = 0; a < fa.n_acc; a++) acc[a] = fa.init[a];
+  u64 st[DBSP_MAX_STACK];
+  for (u64 r = i; r < n; r++) {
+    bool same = true;
+    for (int l = 0; l < nk && r > i; l++)
+      if (G.c[l][r] != G.c[l][i]) { same = false; break; }
+    if (!same) break;
+    run_rowfn(fa.step, FoldEnv{G, nk, r, acc, wG[r]}, st);
+    if (st[fa.n_acc])
+      for (int a = 0; a < fa.n_acc; a++) acc[a] = st[a];
+  }
+  run_rowfn(fa.output, FoldEnv{G, nk, i, acc, 0}, st);
+  keep[i] = st[out_nv] != 0;
+  for (int l = 0; l < out_nv; l++) out.c[l][i] = st[l];
+}
+
 // Max / Min.  Per key, a walk over the union of the spine batches' value lists from the extreme end — the
 // CursorList walk of max.rs:36-55 (backwards from the end) / min.rs:38-57 (forwards): per batch a cursor into the
 // key's value range; the candidate is the extreme value under the cursors, its weight the sum over the batches that
@@ -1243,6 +1299,43 @@ static int32_t distinct_keys(Ctx* ctx, const Batch* b, int nk, Batch** out) {
   return compact_ordered(ctx, ks, b->cols(), b->w, flags, b->n, out);
 }
 
+// The stages of AggregateIncremental::eval + Upsert::eval that every aggregator shares
+// (operator/aggregate/mod.rs:479-547,600-684; operator/upsert.rs:161-208).
+// 2b. the keys' value groups: in_tr's rows of `keys` (nk lanes), weights summed over the batches, zeros dropped
+static int32_t gather_groups(Ctx* ctx, const Batch* keys, int nk, const Spine* in_tr, Batch** G) {
+  return probe_spine(ctx, keys, nk, in_tr, (const dbsp_proj*)nullptr, 1, in_tr->s, G);
+}
+// 3. rows (key lanes `key`, new value lanes `vals`) with weight +1 where keep[i] != 0, in row order
+static int32_t new_values(Ctx* ctx, const dbsp_schema& os, const u64* const* key, const MCols& vals, const u32* keep,
+                          u64 n, Batch** N) {
+  const int nk = os.n_key_lanes, nov = os.n_val_lanes;
+  Cols src;
+  for (int l = 0; l < MAXL; l++) src.c[l] = nullptr;
+  for (int l = 0; l < nk; l++) src.c[l] = key[l];
+  for (int l = 0; l < nov; l++) src.c[nk + l] = vals.c[l];
+  BufP ones;
+  TRY(dev_alloc(ctx, (size_t)n * 8, &ones));
+  k_fill_i64<<<blocks(n), TB, 0, ctx->stream>>>((i64*)ones->p, n, 1);
+  LAUNCH_COUNT(ctx);
+  return compact_ordered(ctx, os, src, (const i64*)ones->p, keep, n, N);
+}
+// 4-5. the keys' current values in the output trace, negated, merged with the new ones (consolidate(+new, -old) per
+// key == merge of two consolidated batches).  Takes `keys` and `N`.
+static int32_t upsert_keys(Ctx* ctx, Batch* keys, Batch* N, const Spine* out_tr, Batch** out) {
+  Batch* O = nullptr;
+  int32_t rc = probe_spine(ctx, keys, out_tr->s.n_key_lanes, out_tr, (const dbsp_proj*)nullptr, 1, out_tr->s, &O);
+  batch_unref(keys);
+  if (rc) { batch_unref(N); return rc; }
+  Batch* On = nullptr;
+  rc = op_neg(ctx, O, &On);
+  batch_unref(O);
+  if (rc) { batch_unref(N); return rc; }
+  rc = merge_batches(ctx, N, On, out);
+  batch_unref(N);
+  batch_unref(On);
+  return rc;
+}
+
 // AggregateIncremental::eval + Upsert::eval
 // (operator/aggregate/mod.rs:479-547,600-684; operator/upsert.rs:161-208).
 int32_t op_aggregate_delta(Ctx* ctx, const Batch* delta, const Spine* in_tr, const Spine* out_tr, int kind, Batch** out) {
@@ -1283,22 +1376,14 @@ int32_t op_aggregate_delta(Ctx* ctx, const Batch* delta, const Spine* in_tr, con
     u64 nslow;
     TRY(read_back(ctx, slow, 1, &nslow));
     if (nslow == 0) {
-      Cols src;
-      for (int l = 0; l < MAXL; l++) src.c[l] = nullptr;
-      for (int l = 0; l < nk; l++) src.c[l] = keys->col[l];
-      for (int l = 0; l < nov; l++) src.c[nk + l] = nvr.c.c[l];
-      BufP ones;
-      TRY(dev_alloc(ctx, (size_t)keys->n * 8, &ones));
-      k_fill_i64<<<blocks(keys->n), TB, 0, st>>>((i64*)ones->p, keys->n, 1);
-      LAUNCH_COUNT(ctx);
-      rc = compact_ordered(ctx, os, src, (const i64*)ones->p, (u32*)kb->p, keys->n, &N);
+      rc = new_values(ctx, os, keys->col, nvr.c, (u32*)kb->p, keys->n, &N);
       if (rc) { batch_unref(keys); return rc; }
     }
   }
   // 2b. general path: the keys' value groups, weights summed over batches
   Batch* G = nullptr;
   if (!N) {
-    rc = probe_spine(ctx, keys, nk, in_tr, (const dbsp_proj*)nullptr, 1, in_tr->s, &G);
+    rc = gather_groups(ctx, keys, nk, in_tr, &G);
     if (rc) { batch_unref(keys); return rc; }
   }
   // 3. aggregate per key -> rows (key, new value) with weight +1
@@ -1319,36 +1404,54 @@ int32_t op_aggregate_delta(Ctx* ctx, const Batch* delta, const Spine* in_tr, con
     TRY(tmp_alloc(ctx, nov, G->n, &nv));
     k_agg_pick<<<blocks(G->n + 1), TB, 0, st>>>(G->cols(), G->w, G->n, gnk, gnv, kind, psum, G->flips(), keep, nv.c, nov);
     LAUNCH_COUNT(ctx);
-    // rows (key lanes of G, new value lanes), weight +1 (reuse delta-free ones array: build below)
-    Cols src;
-    for (int l = 0; l < MAXL; l++) src.c[l] = nullptr;
-    for (int l = 0; l < nk; l++) src.c[l] = G->col[l];
-    for (int l = 0; l < nov; l++) src.c[nk + l] = nv.c.c[l];
-    // weights: all +1
-    BufP ones;
-    TRY(dev_alloc(ctx, (size_t)G->n * 8, &ones));
-    k_fill_i64<<<blocks(G->n), TB, 0, st>>>((i64*)ones->p, G->n, 1);
-    LAUNCH_COUNT(ctx);
-    rc = compact_ordered(ctx, os, src, (const i64*)ones->p, keep, G->n, &N);
+    rc = new_values(ctx, os, G->col, nv.c, keep, G->n, &N);
     if (rc) { batch_unref(keys); batch_unref(G); return rc; }
   } else {
     N = batch_new_empty(ctx, os);
   }
   if (G) batch_unref(G);
-  // 4. current values of those keys in the output trace, negated
-  Batch* O = nullptr;
-  rc = probe_spine(ctx, keys, nk, out_tr, (const dbsp_proj*)nullptr, 1, os, &O);
-  batch_unref(keys);
-  if (rc) { batch_unref(N); return rc; }
-  // 5. consolidate(+new, -old) per key == merge of two consolidated batches
-  Batch* On = nullptr;
-  rc = op_neg(ctx, O, &On);
-  batch_unref(O);
-  if (rc) { batch_unref(N); return rc; }
-  rc = merge_batches(ctx, N, On, out);
-  batch_unref(N);
-  batch_unref(On);
-  return rc;
+  return upsert_keys(ctx, keys, N, out_tr, out);
+}
+
+// AggregateIncremental::eval + Upsert::eval with a Fold (operator/aggregate/fold.rs:60-75): the stages above, with
+// k_agg_fold as the per-key pick.  A key's walk is serial (Fold is not associative, UnimplementedSemigroup).
+int32_t op_aggregate_fold(Ctx* ctx, const Batch* delta, const Spine* in_tr, const Spine* out_tr, const dbsp_fold* fold,
+                          Batch** out) {
+  const dbsp_schema& os = out_tr->s;
+  const int nk = os.n_key_lanes, nov = os.n_val_lanes;
+  if (delta->n == 0) { *out = batch_new_empty(ctx, os); return DBSP_OK; }
+  Batch* keys = nullptr;
+  TRY(distinct_keys(ctx, delta, nk, &keys));
+  Batch* G = nullptr;
+  int32_t rc = gather_groups(ctx, keys, nk, in_tr, &G);
+  if (rc) { batch_unref(keys); return rc; }
+  Batch* N = nullptr;
+  if (G->n) {
+    FoldArgs fa;
+    memset(&fa, 0, sizeof(fa));
+    fa.step = dbsp_validate::fold_step_rowfn(*fold);
+    fa.output = fold->output;
+    fa.n_acc = fold->n_acc;
+    for (int a = 0; a < fold->n_acc; a++) fa.init[a] = fold->init[a];
+    BufP kb;
+    TmpRows nv;
+    rc = dev_alloc(ctx, (size_t)(G->n + 1) * 4, &kb);
+    if (rc == DBSP_OK) rc = tmp_alloc(ctx, nov, G->n, &nv);
+    if (rc == DBSP_OK) {
+      {
+        // G's rows (lanes and weight) read once; each affected key's output lanes written once
+        ProfScope ps(ctx, KID_AGG_FOLD, G->n * (u64)(G->nl() + 1) * 8 + keys->n * (u64)nov * 8);
+        k_agg_fold<<<blocks(G->n + 1), TB, 0, ctx->stream>>>(G->cols(), G->w, G->n, nk, fa, (u32*)kb->p, nv.c, nov);
+      }
+      LAUNCH_COUNT(ctx);
+      rc = new_values(ctx, os, G->col, nv.c, (u32*)kb->p, G->n, &N);
+    }
+  } else {
+    N = batch_new_empty(ctx, os);
+  }
+  batch_unref(G);
+  if (rc) { batch_unref(keys); return rc; }
+  return upsert_keys(ctx, keys, N, out_tr, out);
 }
 
 int32_t op_neg(Ctx* ctx, const Batch* a, Batch** out) {

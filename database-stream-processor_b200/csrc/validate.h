@@ -6,6 +6,7 @@
 // otherwise the text for dbsp_last_error, which names the call (`what`) and the argument.
 #pragma once
 #include <stdint.h>
+#include <string.h>
 
 #include <string>
 
@@ -91,22 +92,30 @@ inline int rowfn_arity(uint8_t op) {
   if (op <= DBSP_FN_LNOT) return 1;
   return op == DBSP_FN_SELECT ? 3 : 2;
 }
+// The source kinds beyond KEY / LVAL / RVAL / CONST a call lets a PUSH take (valid_rowfn's `extra`)
+constexpr unsigned SRC_BIT_FANOUT = 1u << DBSP_SRC_FANOUT, SRC_BIT_ACC = 1u << DBSP_SRC_ACC,
+                   SRC_BIT_WEIGHT = 1u << DBSP_SRC_WEIGHT;
 // A row function: the instructions fit the array, every op and PUSH source is valid for the call (lanes as in
 // valid_src), the stack never underflows or exceeds DBSP_MAX_STACK, and it ends with the output lanes + the keep flag.
-// One pass over the program, so the depth at each instruction is known before any row is evaluated.  `fanout`: the
-// program belongs to a `_fanout` call, where a PUSH may also take DBSP_SRC_FANOUT (j; idx and cst ignored).
+// One pass over the program, so the depth at each instruction is known before any row is evaluated.  `extra`: the
+// further source kinds a PUSH may take (SRC_BIT_*): DBSP_SRC_FANOUT in a `_fanout` call (j; idx and cst ignored),
+// DBSP_SRC_ACC (word idx < n_acc) and DBSP_SRC_WEIGHT (idx and cst ignored) in a fold's programs.  `end` >= 0: the
+// depth the program must end with instead (a fold's step: its n_acc words + the keep flag).  `arg` names the program.
 inline std::string valid_rowfn(const dbsp_rowfn* f, int nk, int n_lval, int n_rval, const std::string& what,
-                               bool fanout = false) {
-  if (!f) return what + ": fn is NULL";
-  std::string m = valid_schema(&f->out_schema, what, "fn.out_schema");
+                               unsigned extra = 0, int n_acc = 0, int end = -1, const std::string& arg = "fn") {
+  if (!f) return what + ": " + arg + " is NULL";
+  std::string m = valid_schema(&f->out_schema, what, (arg + ".out_schema").c_str());
   if (!m.empty()) return m;
-  if (f->n_insn > DBSP_MAX_INSNS) return what + ": fn.n_insn = " + num(f->n_insn) + " exceeds " + num(DBSP_MAX_INSNS);
+  if (f->n_insn > DBSP_MAX_INSNS) return what + ": " + arg + ".n_insn = " + num(f->n_insn) + " exceeds " + num(DBSP_MAX_INSNS);
   int depth = 0;
   for (int i = 0; i < f->n_insn; i++) {
     const dbsp_insn& in = f->code[i];
-    const std::string where = what + ": fn.code[" + num(i) + "]";
+    const std::string where = what + ": " + arg + ".code[" + num(i) + "]";
     if (in.op > DBSP_FN_SELECT) return where + ".op = " + num(in.op) + " is not an instruction";
-    if (in.op == DBSP_FN_PUSH && !(fanout && in.kind == DBSP_SRC_FANOUT)) {
+    const bool allowed = in.kind < 32 && ((extra >> in.kind) & 1);
+    if (in.op == DBSP_FN_PUSH && allowed && in.kind == DBSP_SRC_ACC && in.idx >= n_acc)
+      return where + ".idx = " + num(in.idx) + ": SRC_ACC has " + num(n_acc) + " words";
+    if (in.op == DBSP_FN_PUSH && !allowed) {
       dbsp_src s;
       s.kind = in.kind;
       s.idx = in.idx;
@@ -120,8 +129,10 @@ inline std::string valid_rowfn(const dbsp_rowfn* f, int nk, int n_lval, int n_rv
     if (depth > DBSP_MAX_STACK) return where + ": stack deeper than " + num(DBSP_MAX_STACK);
   }
   const int L = f->out_schema.n_key_lanes + f->out_schema.n_val_lanes;
-  if (depth != L + 1)
-    return what + ": fn ends with stack depth " + num(depth) + ", needs " + num(L + 1) + " (the output lanes, then the keep flag)";
+  if (end >= 0 && depth != end)
+    return what + ": " + arg + " ends with stack depth " + num(depth) + ", needs " + num(end) + " (the accumulator words, then the keep flag)";
+  if (end < 0 && depth != L + 1)
+    return what + ": " + arg + " ends with stack depth " + num(depth) + ", needs " + num(L + 1) + " (the output lanes, then the keep flag)";
   return "";
 }
 // columns of a raw table a row function reads (bit l = column l); call after valid_rowfn
@@ -169,6 +180,43 @@ inline std::string valid_aggregate(const dbsp_schema& delta, const dbsp_schema& 
   if (out.n_val_lanes != 1) return what + ": this agg_kind writes one value lane to out_trace";
   if (kind == DBSP_AGG_WCOUNT ? nv != 0 : nv == 0)
     return what + (kind == DBSP_AGG_WCOUNT ? ": AGG_WCOUNT needs a delta without value lanes" : ": AGG_FOLD_* need a delta with value lanes");
+  return "";
+}
+
+// A fold's step as a dbsp_rowfn (its code, and a one-lane out_schema that only valid_schema reads: the step's end
+// depth is n_acc + 1, given to valid_rowfn as `end`), so that one validator and one interpreter run both programs.
+// Call with n_step <= DBSP_MAX_INSNS.
+inline dbsp_rowfn fold_step_rowfn(const dbsp_fold& f) {
+  dbsp_rowfn r;
+  memset(&r, 0, sizeof(r));
+  r.out_schema.n_val_lanes = 1;
+  r.n_insn = f.n_step;
+  memcpy(r.code, f.step, sizeof(dbsp_insn) * f.n_step);
+  return r;
+}
+
+// aggregate_fold: what aggregate_delta needs of delta / in_trace, the two programs, and an out_trace of delta's key
+// lanes followed by exactly the output program's value lanes.
+inline std::string valid_fold(const dbsp_schema& delta, const dbsp_schema& in, const dbsp_schema& out, const dbsp_fold* f) {
+  const std::string what = "aggregate_fold";
+  if (!f) return what + ": fold is NULL";
+  if (f->n_acc < 1 || f->n_acc > DBSP_MAX_ACC)
+    return what + ": fold.n_acc = " + num(f->n_acc) + ": an accumulator has 1.." + num(DBSP_MAX_ACC) + " words";
+  if (f->n_step > DBSP_MAX_INSNS) return what + ": fold.n_step = " + num(f->n_step) + " exceeds " + num(DBSP_MAX_INSNS);
+  const dbsp_rowfn step = fold_step_rowfn(*f);
+  std::string m = valid_rowfn(&step, delta.n_key_lanes, delta.n_val_lanes, delta.n_val_lanes, what,
+                              SRC_BIT_ACC | SRC_BIT_WEIGHT, f->n_acc, f->n_acc + 1, "fold.step");
+  if (!m.empty()) return m;
+  m = valid_rowfn(&f->output, delta.n_key_lanes, 0, 0, what, SRC_BIT_ACC, f->n_acc, -1, "fold.output");
+  if (!m.empty()) return m;
+  const dbsp_schema& os = f->output.out_schema;
+  if (os.n_key_lanes != 0) return what + ": fold.output.out_schema has key lanes; the output is the key's value lanes only";
+  if (!same_schema(delta, in)) return what + ": delta and in_trace differ in schema";
+  if (!same_key_lanes(delta, out)) return what + ": delta and out_trace differ in key lanes";
+  if (out.n_val_lanes != os.n_val_lanes) return what + ": out_trace must have fold.output's value lanes (count and type)";
+  for (int l = 0; l < os.n_val_lanes; l++)
+    if (out.lane_types[out.n_key_lanes + l] != os.lane_types[l])
+      return what + ": out_trace must have fold.output's value lanes (count and type)";
   return "";
 }
 

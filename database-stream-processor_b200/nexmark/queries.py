@@ -1,4 +1,4 @@
-"""Nexmark q0 / q1 / q2 / q3 / q4 / q7, and q5 as its SQL states it (q5_hop), on the Stream API.
+"""Nexmark q0 / q1 / q2 / q3 / q4 / q6 / q7 / q18, and q5 as its SQL states it (q5_hop), on the Stream API.
 
 The reference's `NexmarkStream` is one stream of `Event` enum rows
 (crates/nexmark/src/queries/mod.rs:12); here it is three column tables
@@ -9,8 +9,8 @@ from __future__ import annotations
 
 from dataclasses import dataclass
 
-from ..circuit import Max, Min, RootCircuit, Stream, TableStream
-from ..zset import Proj, Schema, col, const, fanout_index, key, lval, rval
+from ..circuit import Fold, Max, Min, RootCircuit, Stream, TableStream
+from ..zset import Proj, Schema, acc, col, const, fanout_index, key, lval, rval
 
 WATERMARK_INTERVAL_SECONDS = 4  # queries/mod.rs:12
 TUMBLE_SECONDS = 10             # queries/q7.rs:43
@@ -18,6 +18,7 @@ CATEGORY_OF_INTEREST = 10       # queries/q3.rs:31
 AUCTION_ID_MODULO = 123         # queries/q2.rs:21
 HOP_SLIDE_MS = 2_000            # queries/q5.rs:24-60: HOP(dateTime, INTERVAL '2' SECOND, INTERVAL '10' SECOND)
 HOP_SIZE_MS = 10_000
+NUM_AUCTIONS_PER_SELLER = 10    # queries/q6.rs:39
 
 
 @dataclass
@@ -118,4 +119,33 @@ def q5_hop(inp: NexmarkTables) -> Stream:
     return auction_bids.join(max_bids, Proj(Schema("ui"), [lval(0), lval(1)], where=[lval(1).ge(rval(0)).signed()]))
 
 
-QUERIES = {"q0": q0, "q1": q1, "q2": q2, "q3": q3, "q4": q4, "q7": q7, "q5_hop": q5_hop}
+def q6(inp: NexmarkTables) -> Stream:
+    """queries/q6.rs:41-107: per seller, the average winning price of its last 10 auctions (by auction id), as
+    (seller, avg), u64 division."""
+    # (a.id, (a.seller, a.date_time, a.expires)) and (b.auction, (b.price, b.date_time))  (q6.rs:43-52)
+    auctions_by_id = inp.auction.flat_map_index(Proj(Schema("u", "uuu"), [col(0), col(1), col(3), col(4)]))
+    bids_by_auction = inp.bid.flat_map_index(Proj(Schema("u", "uu"), [col(0), col(2), col(3)]))
+    # ((auction_id, seller), bid_price) for bids inside [date_time, expires]  (q6.rs:58-79)
+    bids_for_auctions = auctions_by_id.join_index(
+        bids_by_auction,
+        Proj(Schema("uu", "u"), [key(0), lval(0), rval(0)], where=[rval(1).ge(lval(1)), rval(1).le(lval(2))]))
+    # seller -> (auction, winning price)  (q6.rs:86-88)
+    winning = bids_for_auctions.aggregate(Max).map_index(Proj(Schema("u", "uu"), [key(1), key(0), lval(0)]))
+    # the VecDeque of the last 10 prices as words 0..9, newest in word 9 (words of a deque shorter than 10 that were
+    # never pushed stay 0), and its length in word 10  (q6.rs:93-106)
+    n = NUM_AUCTIONS_PER_SELLER
+    last_prices = Fold([0] * (n + 1), [acc(i + 1) for i in range(n - 1)] + [lval(1), (acc(n) + 1).min(n)],
+                       output=Proj(Schema("", "u"), [sum((acc(i) for i in range(1, n)), acc(0)).divu(acc(n))]))
+    return winning.aggregate(last_prices)
+
+
+def q18(inp: NexmarkTables) -> Stream:
+    """queries/q18.rs:37-50: the last bid (latest date_time) of every (auction, bidder).  The accumulator starts as
+    Bid::default() (zeros) and takes a value iff its date_time is strictly later, so of two bids at one date_time the
+    first in value order wins."""
+    bids = inp.bid.flat_map_index(Proj(Schema("uu", "uuuuu"), [col(0), col(1), col(0), col(1), col(2), col(3), col(4)]))
+    last = Fold([0] * 5, [key(0), key(1), lval(2), lval(3), lval(4)], where=lval(3).gt(acc(3)))
+    return bids.aggregate(last).map(Proj(Schema("uuuuu"), [lval(i) for i in range(5)]))
+
+
+QUERIES = {"q0": q0, "q1": q1, "q2": q2, "q3": q3, "q4": q4, "q7": q7, "q5_hop": q5_hop, "q6": q6, "q18": q18}

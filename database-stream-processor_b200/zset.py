@@ -19,7 +19,7 @@ from typing import Iterable, Sequence
 import numpy as np
 
 from . import _capi as capi
-from ._capi import CApi, CExpr, CPred, CProj, CRowFn, CSchema, CSrc, as_u64, col_ptrs
+from ._capi import CApi, CExpr, CFold, CPred, CProj, CRowFn, CSchema, CSrc, as_u64, col_ptrs
 
 
 @dataclass(frozen=True)
@@ -245,6 +245,16 @@ def fanout_index():
     return Src(capi.SRC_FANOUT)
 
 
+def acc(i):
+    """word i of a Fold's accumulator (its step and output programs only)"""
+    return Src(capi.SRC_ACC, i)
+
+
+def weight():
+    """the weight of the value a Fold's step is applied to (summed over the trace's batches), as i64 bits"""
+    return Src(capi.SRC_WEIGHT)
+
+
 def where_(c, a, b):
     """`if c { a } else { b }` (c non-zero = true)"""
     return Fn(capi.FN_SELECT, c, a, b)
@@ -344,6 +354,24 @@ def _i64(c):
 
 def compile_rowfn(schema: Schema, out: Sequence, where: Sequence = ()) -> CRowFn:
     """The postfix program of a closure: the output lanes in order, then the keep flag (the AND of `where`)."""
+    code = _compile_code(out, where)
+    f = CRowFn()
+    f.out_schema = schema.c()
+    f.n_insn = len(code)
+    for i, (op, kind, idx, cst) in enumerate(code):
+        f.code[i].op, f.code[i].kind, f.code[i].idx, f.code[i].cst = op, kind, idx, _i64(cst)
+    return f
+
+
+def compile_fold_step(step: Sequence, where: Sequence = ()) -> list:
+    """A Fold's step program: its n_acc (1 .. MAX_ACC) new accumulator words in order, then the keep flag (the AND of
+    `where`).  The words are untyped, so no schema bounds them; the stack holds n_acc + 1 <= MAX_STACK values."""
+    if not 1 <= len(step) <= capi.MAX_ACC:
+        raise ValueError(f"Fold: the step gives {len(step)} accumulator words; an accumulator has 1..{capi.MAX_ACC}")
+    return _compile_code(step, where)
+
+
+def _compile_code(out: Sequence, where: Sequence) -> list:
     code = []
     for o in out:
         _val(o).emit(code)
@@ -358,11 +386,17 @@ def compile_rowfn(schema: Schema, out: Sequence, where: Sequence = ()) -> CRowFn
             code.append((capi.FN_AND, 0, 0, 0))
     if len(code) > capi.MAX_INSNS:
         raise ValueError(f"the closure needs {len(code)} instructions; a row function has at most {capi.MAX_INSNS}")
-    f = CRowFn()
-    f.out_schema = schema.c()
-    f.n_insn = len(code)
-    for i, (op, kind, idx, cst) in enumerate(code):
-        f.code[i].op, f.code[i].kind, f.code[i].idx, f.code[i].cst = op, kind, idx, _i64(cst)
+    return code
+
+
+def compile_fold(init: Sequence[int], step_code: list, output: CRowFn) -> CFold:
+    f = CFold()
+    f.n_acc, f.n_step = len(init), len(step_code)
+    for i, x in enumerate(init):
+        f.init[i] = int(x) & ((1 << 64) - 1)
+    for i, (op, kind, idx, cst) in enumerate(step_code):
+        f.step[i].op, f.step[i].kind, f.step[i].idx, f.step[i].cst = op, kind, idx, _i64(cst)
+    f.output = output
     return f
 
 
@@ -924,6 +958,12 @@ class Backend:
     def aggregate_delta(self, delta: Batch, in_trace: Spine, out_trace: Spine, kind: int) -> Batch:
         out = self._out()
         self.api.call("aggregate_delta", self.ctx, delta.h, in_trace.h, out_trace.h, kind, C.byref(out))
+        return Batch(self, out.value, out_trace.schema)
+
+    def aggregate_fold(self, delta: Batch, in_trace: Spine, out_trace: Spine, fold) -> Batch:
+        """aggregate_delta with a Fold (circuit.Fold, or anything with a CFold `_c`) as the aggregator."""
+        out = self._out()
+        self.api.call("aggregate_fold", self.ctx, delta.h, in_trace.h, out_trace.h, C.byref(fold._c), C.byref(out))
         return Batch(self, out.value, out_trace.schema)
 
     def weigh(self, b: Batch, f, mode: int) -> Batch:

@@ -85,10 +85,15 @@ enum dbsp_src_kind {
   DBSP_SRC_RVAL = 2,  /* lane `idx` of the right value (v2 of join_func);
                          in a call with one input: the same lanes as LVAL  */
   DBSP_SRC_CONST = 3, /* the constant `cst`                                 */
-  DBSP_SRC_FANOUT = 4 /* row functions of the `_fanout` calls only: j, the
+  DBSP_SRC_FANOUT = 4,/* row functions of the `_fanout` calls only: j, the
                          index (0 .. n_out-1) of the output being generated;
                          idx and cst are ignored.  Every other call refuses
                          it as outside the enum.                            */
+  DBSP_SRC_ACC = 5,   /* the programs of a dbsp_fold only: accumulator word
+                         `idx` (< n_acc)                                     */
+  DBSP_SRC_WEIGHT = 6 /* a dbsp_fold's step only: the value's weight (summed
+                         over the trace's batches) as i64 bits; idx and cst
+                         are ignored                                         */
 };
 enum dbsp_expr_op {
   DBSP_OP_COPY = 0, DBSP_OP_NEG = 1, DBSP_OP_ADD = 2, DBSP_OP_SUB = 3,
@@ -171,6 +176,27 @@ typedef struct dbsp_rowfn {
   uint8_t pad_[5];
   dbsp_insn code[DBSP_MAX_INSNS];
 } dbsp_rowfn;
+
+/* A Fold aggregator (operator/aggregate/fold.rs: Fold::new / with_output) as
+ * two row-function programs over an accumulator of n_acc untyped u64 words:
+ *   init    the accumulator's first value (Fold::init; words >= n_acc unused);
+ *   step    Fold::step(&mut acc, &value, weight), n_step instructions over
+ *           KEY / LVAL (RVAL = LVAL) of the value's row, ACC, WEIGHT and
+ *           CONST; it ends with the n_acc new words, then a keep flag: 0 leaves
+ *           acc unchanged, non-zero replaces it with the new words;
+ *   output  Fold's output function, a dbsp_rowfn over KEY, ACC and CONST whose
+ *           out_schema has only value lanes (the aggregate's values); a keep
+ *           flag of 0 gives the key no output row.
+ * The accumulator plus the keep flag fit the DBSP_MAX_STACK-deep stack. */
+#define DBSP_MAX_ACC 15
+typedef struct dbsp_fold {
+  uint8_t n_acc;                    /* 1..DBSP_MAX_ACC */
+  uint8_t n_step;                   /* instructions in step[], <= DBSP_MAX_INSNS */
+  uint8_t pad_[6];
+  uint64_t init[DBSP_MAX_ACC];
+  dbsp_insn step[DBSP_MAX_INSNS];
+  dbsp_rowfn output;
+} dbsp_fold;
 
 /* Aggregators (operator/aggregate/{max,min,fold}.rs, mod.rs:129-156). */
 enum dbsp_agg_kind {
@@ -457,6 +483,20 @@ int32_t dbsp_aggregate_delta(dbsp_ctx* ctx, const dbsp_batch* delta,
                              const dbsp_spine* in_trace,
                              const dbsp_spine* out_trace, int32_t agg_kind,
                              dbsp_batch** out);
+/* The same AggregateIncremental + Upsert with a Fold (fold.rs:60-75) as the
+ * aggregator.  For every key of `delta`, the key's values in `in_trace` are
+ * taken in value order with their weights summed over the batches, and values
+ * whose sum is 0 are skipped.  Starting from fold->init, `step` runs once per
+ * remaining value, serially (Fold is not associative).  A key with at least
+ * one such value gets the row (key, output(acc)) unless output's keep flag is
+ * 0; a key with none gets no row.  The result is -old +new against
+ * `out_trace`, as in dbsp_aggregate_delta.  delta and in_trace have one
+ * schema; out_trace has delta's key lanes followed by fold->output's value
+ * lanes (count and types). */
+int32_t dbsp_aggregate_fold(dbsp_ctx* ctx, const dbsp_batch* delta,
+                            const dbsp_spine* in_trace,
+                            const dbsp_spine* out_trace, const dbsp_fold* fold,
+                            dbsp_batch** out);
 /* weigh (aggregate/mod.rs:297-323). `f` gives f(k,v) (SRC_KEY/SRC_LVAL).
  * `mode` is a dbsp_weigh_mode; WEIGH_AVG adds a key lane (at most 7 before). */
 int32_t dbsp_weigh(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_expr* f,

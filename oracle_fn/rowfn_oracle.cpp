@@ -1,8 +1,9 @@
 // rowfn_oracle.cpp — the CPU oracle with row functions (dbsp_rowfn, include/dbsp_b200.h): the whole oracle of
-// oracle/dbsp_oracle.cpp, unchanged, plus the `_fn` and `_fanout` entry points and dbsp_antijoin_delta, in one translation unit so that they build on its
+// oracle/dbsp_oracle.cpp, unchanged, plus the `_fn` and `_fanout` entry points, dbsp_antijoin_delta and
+// dbsp_aggregate_fold, in one translation unit so that they build on its
 // batches, traces, consolidation and error text.  The oracle's own library stays the checker of every `dbsp_proj`
 // test; this one (libdbsp_oracle_fn.so, test infrastructure like it, never linked into the product) is the checker
-// of the row-function and antijoin tests.  The interpreter below is written apart from the CUDA library's; validate.h is shared,
+// of the row-function, antijoin and fold tests.  The interpreter below is written apart from the CUDA library's; validate.h is shared,
 // so both libraries refuse the same programs with the same texts.
 #include "../oracle/dbsp_oracle.cpp"
 
@@ -10,8 +11,9 @@ namespace {
 
 // The postfix program over a stack; afterwards st[0..L) are the output lanes and st[L] the keep flag.  The arithmetic
 // follows Rust's wrapping_* integer methods with x / 0 = x % 0 = 0 (DESIGN §2).  j: the output a fan-out generates,
-// pushed by DBSP_SRC_FANOUT (validated away everywhere else).
-void run_rowfn(const dbsp_rowfn& f, const Env& e, u64* st, u64 j = 0) {
+// pushed by DBSP_SRC_FANOUT; acc / w: a fold's accumulator and the value's weight, pushed by DBSP_SRC_ACC /
+// DBSP_SRC_WEIGHT (each validated away in the calls that do not have it).
+void run_rowfn(const dbsp_rowfn& f, const Env& e, u64* st, u64 j = 0, const u64* acc = nullptr, i64 w = 0) {
   int sp = 0;
   for (int pc = 0; pc < f.n_insn; pc++) {
     const dbsp_insn& in = f.code[pc];
@@ -20,7 +22,8 @@ void run_rowfn(const dbsp_rowfn& f, const Env& e, u64* st, u64 j = 0) {
       s.kind = in.kind;
       s.idx = in.idx;
       s.cst = in.cst;
-      st[sp++] = in.kind == DBSP_SRC_FANOUT ? j : src_val(s, e);
+      st[sp++] = in.kind == DBSP_SRC_FANOUT ? j : in.kind == DBSP_SRC_ACC ? acc[in.idx] : in.kind == DBSP_SRC_WEIGHT ? (u64)w
+                                                                                                         : src_val(s, e);
       continue;
     }
     const int pops = dbsp_validate::rowfn_arity(in.op);
@@ -111,7 +114,7 @@ void join_into_fn(const Batch& L, const Batch& R, const dbsp_rowfn& f, bool swap
 // n_out == 0: a plain row function (`_fn`); otherwise a fan-out whose program runs for j = 0 .. n_out-1 per row.
 int32_t table_to_batch_fn(const char* what, const u64* const* cols, uint32_t ncols, unsigned col_mask, const i64* w, u64 n,
                           const dbsp_rowfn* fn, orc_batch** out, uint32_t n_out = 0) {
-  REFUSE(dv::valid_rowfn(fn, (int)ncols, (int)ncols, (int)ncols, what, n_out != 0));
+  REFUSE(dv::valid_rowfn(fn, (int)ncols, (int)ncols, (int)ncols, what, n_out != 0 ? dv::SRC_BIT_FANOUT : 0u));
   const unsigned used = dv::rowfn_table_mask(*fn);
   CHECK_ARG((used & ~col_mask) == 0, std::string(what) + ": fn reads column " + std::to_string(__builtin_ctz((used & ~col_mask) | 0x100u)) +
                                          ", which col_mask left out of the upload");
@@ -132,6 +135,33 @@ int32_t table_to_batch_fn(const char* what, const u64* const* cols, uint32_t nco
 std::string valid_join_fn(const char* what, const dbsp_schema& left, const dbsp_schema& right, const dbsp_rowfn* f) {
   if (!dv::same_key_lanes(left, right)) return std::string(what) + ": the two inputs differ in key lanes (count or type)";
   return dv::valid_rowfn(f, left.n_key_lanes, left.n_val_lanes, right.n_val_lanes, what);
+}
+
+// Upsert::eval for one key (operator/upsert.rs:161-208): retract the key's current values in the output trace, insert
+// the new one (if any), and push what does not cancel.
+void upsert_key(Builder& bld, const Spine& out_tr, const u64* key, const u64* newv, bool has_new) {
+  const dbsp_schema& os = out_tr.s;
+  const int nov = os.n_val_lanes;
+  std::vector<std::pair<KV, i64>> grp;
+  key_group(out_tr, key, grp);
+  std::vector<std::pair<std::vector<u64>, i64>> upd;
+  if (has_new) upd.push_back({std::vector<u64>(newv, newv + nov), 1});
+  for (auto& g : grp)
+    if (g.second != 0) {
+      std::vector<u64> v(nov);
+      g.first.b->V.get(g.first.pos, v.data());
+      upd.push_back({v, (i64)((u64)0 - (u64)g.second)});
+    }
+  const uint8_t* vty = os.lane_types + os.n_key_lanes;
+  std::sort(upd.begin(), upd.end(), [&](auto& a, auto& b) { return cmp_tuples(vty, nov, a.first.data(), b.first.data()) < 0; });
+  for (size_t i = 0; i < upd.size();) {
+    size_t j = i;
+    i64 sum = 0;
+    for (; j < upd.size() && cmp_tuples(vty, nov, upd[i].first.data(), upd[j].first.data()) == 0; j++)
+      sum = (i64)((u64)sum + (u64)upd[j].second);
+    if (sum != 0) bld.push(key, upd[i].first.data(), sum);
+    i = j;
+  }
 }
 
 }  // namespace
@@ -225,8 +255,49 @@ int32_t orc_antijoin_delta(orc_ctx* c, const orc_batch* delta, const orc_spine* 
   return DBSP_OK;
 }
 
+// AggregateIncremental + Upsert with a Fold, as fold.rs:60-75 reads: per key of delta, the key's values in value
+// order with their weights summed over the batches; a value of weight 0 is skipped, every other one runs `step`
+// (whose keep flag decides whether its words become the accumulator); a non-empty key's output row is output(acc)
+// unless the output program drops it.  Written apart from the CUDA library's gather and per-key walk.
+int32_t orc_aggregate_fold(orc_ctx* c, const orc_batch* delta, const orc_spine* in_tr, const orc_spine* out_tr,
+                           const dbsp_fold* fold, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(delta, "delta");
+  NOT_NULL(in_tr, "in_trace");
+  NOT_NULL(out_tr, "out_trace");
+  REFUSE(dv::valid_fold(delta->p->s, in_tr->s.s, out_tr->s.s, fold));
+  const Batch& D = *delta->p;
+  const int n_acc = fold->n_acc, nov = out_tr->s.s.n_val_lanes;
+  const dbsp_rowfn step = dv::fold_step_rowfn(*fold);
+  Builder bld(out_tr->s.s);
+  std::vector<std::pair<KV, i64>> grp;
+  u64 key[MAXL], val[MAXL] = {0}, acc[DBSP_MAX_ACC], st[DBSP_MAX_STACK];
+  for (size_t k = 0; k < D.K.n; k++) {
+    D.K.get(k, key);
+    key_group(in_tr->s, key, grp);
+    std::copy(fold->init, fold->init + n_acc, acc);
+    bool non_empty = false;
+    for (auto& g : grp) {
+      if (g.second == 0) continue;
+      non_empty = true;
+      if (g.first.b->indexed()) g.first.b->V.get(g.first.pos, val);
+      run_rowfn(step, Env{key, val, val}, st, 0, acc, g.second);
+      if (st[n_acc] != 0) std::copy(st, st + n_acc, acc);
+    }
+    bool has_new = false;
+    if (non_empty) {
+      run_rowfn(fold->output, Env{key, val, val}, st, 0, acc, 0);
+      has_new = st[nov] != 0;
+    }
+    upsert_key(bld, out_tr->s, key, st, has_new);
+  }
+  *out = wrap(bld.done());
+  return DBSP_OK;
+}
+
 uint32_t orc_fanout_table_mask(const dbsp_rowfn* fn) {
-  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "fanout_table_mask", true).empty()) return 0;
+  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "fanout_table_mask", dv::SRC_BIT_FANOUT).empty()) return 0;
   return dv::rowfn_table_mask(*fn);
 }
 
@@ -299,7 +370,7 @@ int32_t orc_weigh_fn(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* f, int32_
 // Map/FlatMap/Index::eval + from_tuples (operator/filter_map.rs:563-577,700-724); n_out == 0: no fan-out.
 static int32_t map_index_fn(const char* what, const orc_batch* b, const dbsp_rowfn* fn, uint32_t n_out, orc_batch** out) {
   const Batch& B = *b->p;
-  REFUSE(dv::valid_rowfn(fn, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, what, n_out != 0));
+  REFUSE(dv::valid_rowfn(fn, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, what, n_out != 0 ? dv::SRC_BIT_FANOUT : 0u));
   FANOUT_ROWS(B.indexed() ? B.V.n : B.K.n, n_out, what);
   Tuples t(fn->out_schema);
   u64 key[MAXL], val[MAXL] = {0}, row[MAXL];

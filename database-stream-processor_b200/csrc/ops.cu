@@ -331,33 +331,115 @@ k_project_rows(Cols in, int nk_in, const i64* w, u64 n, F proj, int identity, u3
 }
 
 // ---------------- delta x trace probes -----------------------------------------
-// Per *distinct* delta key (delta rows are sorted, so a key's rows are one
-// segment [kstart[k], kstart[k+1])) and per trace batch: the range of trace rows
-// carrying that key — lower bound by bisection, upper bound by galloping (the
-// `seek_key` of cursor/mod.rs + advance.rs:25-72).  One search per key instead of
-// one per row; all spine batches in one launch.
-__global__ void k_probe_keys(Cols D, const u64* kstart, const u32* d_nkeys, BatchRefs tr, int nk, Flips f, u32* lo_out,
-                             u32* cnt_out, u32* ktot) {
-  const u64 gtid = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+// Warp range search: the rows of 32 consecutive distinct sorted query keys (one per lane) in each batch of a launch.
+// Most probes touch few batches (ids grow from step to step, so a step's keys sit in the newest batches or above
+// all of them), and a thread walking every batch alone runs ~log2(n) dependent loads per batch.  Instead:
+// - bounds test: the first and last key of every batch sit in shared memory; a batch that the warp's key span
+//   [q_min, q_max] misses is skipped by the whole warp without a global load;
+// - shared window: the warp narrows [lower_bound(q_min), upper_bound(q_max)) together, 32 pivots per round and a
+//   ballot per bound, so a window shrinks ~32x per round of independent loads;
+// - per lane: lower bound by bisection inside that window, upper bound by galloping (the `seek_key` of
+//   cursor/mod.rs + advance.rs:25-72) capped at the window's end.
+// The search is exact: a key with rows in a batch gets its lower bound and count there.  A key without rows gets
+// hi == lo and an unspecified lo: no caller reads lo for an empty range.
+// The shared window stops narrowing at this width: a round's pivots are then spread over every warp of the launch
+// and miss the cache, so a round costs more than the bisection steps it saves the lanes (random keys, 10 M-row
+// batches, measured on an H100).
+constexpr u64 WIN_MIN = 1024;
+struct BatchBounds {
+  u64 first[MAX_REFS][MAXL], last[MAX_REFS][MAXL];   // flipped like the queries; unset for an empty batch
+  u64 q[TB / 32][2][MAXL];                            // per warp: its smallest and its largest query key
+};
+// every thread of the block calls it (it ends in a barrier)
+__device__ __forceinline__ void load_bounds(BatchBounds& s, const BatchRefs& tr, int nk, const Flips& f) {
+  for (int i = threadIdx.x; i < tr.nb * 2 * nk; i += blockDim.x) {
+    const int b = i / (2 * nk), l = i % nk;
+    const bool last = i % (2 * nk) >= nk;
+    const u64 n = tr.b[b].n;
+    if (n) (last ? s.last : s.first)[b][l] = tr.b[b].c.c[l][last ? n - 1 : 0] ^ f.f[l];
+  }
+  __syncthreads();
+}
+__device__ __forceinline__ int cmp_keys(const u64* a, const u64* b, int nk) {
+  for (int l = 0; l < nk; l++)
+    if (a[l] != b[l]) return a[l] < b[l] ? -1 : 1;
+  return 0;
+}
+// Lanes [0, nact) hold the warp's keys in ascending order, q of an idle lane is not read.  Publishes the warp's key
+// span for warp_key_range; every lane calls it.
+__device__ __forceinline__ void warp_key_span(BatchBounds& s, const u64* q, int nact, int nk) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  __syncwarp();   // the previous span's readers are done
+  if (lane == 0) for (int l = 0; l < nk; l++) s.q[wid][0][l] = q[l];
+  if (lane == nact - 1) for (int l = 0; l < nk; l++) s.q[wid][1][l] = q[l];
+  __syncwarp();
+}
+// One round of a 32-ary search for the first row of [a, b) whose predicate holds (b if none): lane j tested the
+// pivot a + j*m/32, m = b - a, and `bal` is the ballot.  The answer stays in [a, b].
+__device__ __forceinline__ void narrow(u64& a, u64& b, u64 m, unsigned bal) {
+  if (m == 0) return;
+  if (!bal) { a += (31 * m >> 5) + 1; return; }
+  const u64 j = (u64)(__ffs(bal) - 1);   // pivot j - 1 < pivot j: equal pivots give equal predicates
+  b = a + (j * m >> 5);
+  if (j) a += ((j - 1) * m >> 5) + 1;
+}
+// [lo, hi) of this lane's key q (flipped) in batch b of s; `active`: the lane holds a key.  Every lane of the warp
+// calls it with the same batch.
+__device__ __forceinline__ void warp_key_range(const BatchBounds& s, const BatchRefs& tr, int b, const u64* q,
+                                               bool active, int nk, const Flips& f, u64& lo, u64& hi) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const u64* qmin = s.q[wid][0];
+  const u64* qmax = s.q[wid][1];
+  const u64 nt = tr.b[b].n;
+  lo = hi = 0;
+  if (nt == 0 || cmp_keys(qmax, s.first[b], nk) < 0 || cmp_keys(qmin, s.last[b], nk) > 0) return;
+  const Cols& T = tr.b[b].c;
+  u64 a0 = 0, b0 = nt, a1 = 0, b1 = nt;   // lower_bound(qmin) in [a0, b0], upper_bound(qmax) in [a1, b1]
+  while (b0 - a0 > WIN_MIN || b1 - a1 > WIN_MIN) {
+    const u64 m0 = b0 - a0, m1 = b1 - a1;
+    const bool g0 = m0 && cmp_row_q(T, a0 + ((u64)lane * m0 >> 5), qmin, nk, f) >= 0;
+    const bool g1 = m1 && cmp_row_q(T, a1 + ((u64)lane * m1 >> 5), qmax, nk, f) > 0;
+    narrow(a0, b0, m0, __ballot_sync(0xffffffffu, g0));
+    narrow(a1, b1, m1, __ballot_sync(0xffffffffu, g1));
+  }
+  if (!active) return;
+  const u64 top = b1;   // every key of the warp lies in rows [a0, b1)
+  lo = lower_bound_q(T, a0, top, q, nk, f);
+  hi = lo;
+  u64 step = 1;
+  while (hi + step <= top && cmp_row_q(T, hi + step - 1, q, nk, f) == 0) { hi += step; step <<= 1; }
+  hi = upper_bound_q(T, hi, hi + step <= top ? hi + step : top, q, nk, f);
+}
+
+// Per *distinct* delta key (delta rows are sorted, so a key's rows are one segment [kstart[k], kstart[k+1])) and
+// per trace batch: the range of trace rows carrying that key.  One search per key instead of one per row; a warp
+// per 32 keys; all spine batches in one launch.
+__global__ void k_probe_keys(Cols D, const u64* kstart, const u32* d_nkeys, BatchRefs tr, int nk, Flips f, u32* lo_out, u32* cnt_out,
+             u32* ktot) {
+  __shared__ BatchBounds s;
+  load_bounds(s, tr, nk, f);
+  const int lane = threadIdx.x & 31;
   const u64 nkeys = (u64)*d_nkeys;   // the exact key count lives on the device; the grid is a fixed-size grid-stride loop
-  for (u64 k = gtid; k < nkeys; k += (u64)gridDim.x * blockDim.x) {
-    const u64 row = kstart[k];
+  for (u64 base = (u64)blockIdx.x * TB + (threadIdx.x & ~31); base < nkeys; base += (u64)gridDim.x * TB) {
+    const u64 k = base + lane;
+    const bool active = k < nkeys;
     u64 q[MAXL];
-    for (int l = 0; l < nk; l++) q[l] = D.c[l][row] ^ f.f[l];
+    if (active) {
+      const u64 row = kstart[k];
+      for (int l = 0; l < nk; l++) q[l] = D.c[l][row] ^ f.f[l];
+    }
+    warp_key_span(s, q, (int)min(nkeys - base, (u64)32), nk);
     u64 tot = 0;
     for (int b = 0; b < tr.nb; b++) {
-      const Cols& T = tr.b[b].c;
-      const u64 nt = tr.b[b].n;
-      u64 lo = lower_bound_q(T, 0, nt, q, nk, f);
-      u64 hi = lo, step = 1;
-      while (hi + step <= nt && cmp_row_q(T, hi + step - 1, q, nk, f) == 0) { hi += step; step <<= 1; }
-      u64 top = hi + step <= nt ? hi + step : nt;
-      hi = upper_bound_q(T, hi, top, q, nk, f);
-      lo_out[k * tr.nb + b] = (u32)lo;
-      cnt_out[k * tr.nb + b] = (u32)(hi - lo);
+      u64 lo, hi;
+      warp_key_range(s, tr, b, q, active, nk, f, lo, hi);
+      if (active) {
+        lo_out[k * tr.nb + b] = (u32)lo;
+        cnt_out[k * tr.nb + b] = (u32)(hi - lo);
+      }
       tot += hi - lo;
     }
-    ktot[k] = tot > 0xffffffffull ? 0xffffffffu : (u32)tot;   // saturate: the 64-bit total below then trips the guard
+    if (active) ktot[k] = tot > 0xffffffffull ? 0xffffffffu : (u32)tot;   // saturate: the 64-bit total below then trips the guard
   }
 }
 
@@ -488,23 +570,27 @@ k_row_counts_scan(const u32* __restrict__ ki, const u32* __restrict__ ktot, u64 
 // needs no sort.  proj_mode 1: join_func(k, v1, v2) with filter
 // (join.rs:751-787), weight w1*w2, rejected rows keep their slot with weight 0;
 // proj_mode 0: copy the trace row (gather of a key group).
-// Load balancing: a CTA owns PF_TILE consecutive output slots whatever the fan-out of the keys behind them
-// (skew-proof).  Two threads bisect the scanned match counts for the delta rows of the tile's first and last
-// slot; the counts in between are staged in shared memory, where every slot finds its delta row — one global
-// bisection per 1024 slots instead of one per slot.  Consecutive slots read consecutive trace rows and
-// the same / adjacent delta rows, and write consecutive output rows.
-constexpr int PF_TILE = 1024, PF_SMEM_ROWS = 3072;
+// Load balancing: a CTA owns `spt` * PF_THREADS consecutive output slots whatever the fan-out of the keys behind them
+// (skew-proof).  Two threads bisect the scanned match counts for the delta rows of the tile's first and last slot;
+// the counts in between are staged in shared memory, where every slot finds its delta row — one global bisection
+// per tile instead of one per slot.  Consecutive slots read consecutive trace rows and the same / adjacent delta
+// rows, and write consecutive output rows.  The host picks the tile from the match count: one slot per thread
+// (spt = 1) spreads a step's few ten thousand matches over every SM; from PF_BIG_TILE_FROM matches on, four slots
+// per thread amortise the tile's bisections over more slots (measured faster at q4's match counts on an H100).
+constexpr int PF_THREADS = 256, PF_SMEM_ROWS = 3072;
+constexpr u64 PF_BIG_TILE_FROM = 1u << 20;
 template <class F>
-__global__ void __launch_bounds__(256)
+__global__ void
 k_probe_fill(Cols D, const i64* wD, u64 nd, BatchRefs tr, int nk, int nvD, int nvT, const u32* lo, const u32* cnt,
-             const u32* ki, const u32* exscan, u64 total, int proj_mode, int delta_is_left, F proj, MCols out,
+             const u32* ki, const u32* exscan, u64 total, int spt, int proj_mode, int delta_is_left, F proj, MCols out,
              i64* out_w) {
   __shared__ u32 s_ex[PF_SMEM_ROWS + 1];
   __shared__ u64 s_rows[2];
   const int tid = threadIdx.x;
-  const u64 o0 = (u64)blockIdx.x * PF_TILE;
+  const u64 tile = (u64)spt * PF_THREADS;
+  const u64 o0 = (u64)blockIdx.x * tile;
   if (o0 >= total) return;
-  const u64 o1 = o0 + PF_TILE < total ? o0 + PF_TILE : total;
+  const u64 o1 = o0 + tile < total ? o0 + tile : total;
   if (tid < 2) {   // largest i with exscan[i] <= target
     const u64 target = tid == 0 ? o0 : o1 - 1;
     u64 a = 0, b = nd;
@@ -519,11 +605,11 @@ k_probe_fill(Cols D, const i64* wD, u64 nd, BatchRefs tr, int nk, int nvD, int n
   const u64 nr = row_hi - row_lo + 1;
   const bool staged = nr <= (u64)PF_SMEM_ROWS;
   if (staged)
-    for (u64 k = tid; k <= nr; k += 256) s_ex[k] = exscan[row_lo + k];
+    for (u64 k = tid; k <= nr; k += PF_THREADS) s_ex[k] = exscan[row_lo + k];
   __syncthreads();
 #pragma unroll 1
-  for (int qq = 0; qq < PF_TILE / 256; qq++) {
-    const u64 o = o0 + (u64)qq * 256 + tid;
+  for (int qq = 0; qq < spt; qq++) {
+    const u64 o = o0 + (u64)qq * PF_THREADS + tid;
     if (o >= o1) break;
     u64 i;
     u32 r;
@@ -545,6 +631,7 @@ k_probe_fill(Cols D, const i64* wD, u64 nd, BatchRefs tr, int nk, int nvD, int n
       r = (u32)(o - exscan[i]);
     }
     const u64 kbase = (u64)ki[i] * tr.nb;
+    // r < the key's total, so the walk stops in a batch with cnt > 0: lo of an empty range (unspecified) is never read
     int bb = 0;
     while (bb < tr.nb - 1 && r >= cnt[kbase + bb]) { r -= cnt[kbase + bb]; bb++; }
     const Cols& T = tr.b[bb].c;
@@ -777,30 +864,28 @@ __global__ void k_agg_fold(Cols G, const i64* wG, u64 n, int nk, FoldArgs fa, u3
 // progress holds +1 and -1 in two batches) steps those cursors and tries the next value.  Keys that need more than
 // AGG_WALK steps are flagged for the general gather path.
 constexpr int AGG_WALK = 64;
-__global__ void k_agg_extremum(Cols K, u64 nkeys, int nk, int nv, BatchRefs tr, Flips f, int is_max, u32* keep,
-                               MCols outv, u64* slow_counter) {
-  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i > nkeys) return;
-  if (i == nkeys) { keep[nkeys] = 0; return; }
+__global__ void k_agg_extremum(Cols K, u64 nkeys, int nk, int nv, BatchRefs tr, Flips f, int is_max, u32* keep, MCols outv,
+               u64* slow_counter) {
+  __shared__ BatchBounds s;
+  load_bounds(s, tr, nk, f);
+  const u64 base = (u64)blockIdx.x * TB + (threadIdx.x & ~31);   // the keys are distinct and sorted: a warp's 32 keys
+  const u64 i = base + (threadIdx.x & 31);
+  if (i == nkeys) keep[nkeys] = 0;
+  if (base >= nkeys) return;   // whole warps only: the range search below takes every lane of a warp
+  const bool active = i < nkeys;
   u64 q[MAXL], best[MAXL];
-  for (int l = 0; l < nk; l++) q[l] = K.c[l][i] ^ f.f[l];
+  if (active)
+    for (int l = 0; l < nk; l++) q[l] = K.c[l][i] ^ f.f[l];
+  warp_key_span(s, q, (int)min(nkeys - base, (u64)32), nk);
   // the key's value range [lo, hi) in every batch; cur = next candidate position
   u32 lo[MAX_REFS], hi[MAX_REFS];
   for (int b = 0; b < tr.nb; b++) {
-    const Cols& T = tr.b[b].c;
-    const u64 nt = tr.b[b].n;
-    const u64 l0 = lower_bound_q(T, 0, nt, q, nk, f);
-    u64 h0 = l0;
-    if (l0 < nt && cmp_row_q(T, l0, q, nk, f) == 0) {
-      u64 step = 1;
-      h0 = l0 + 1;
-      while (h0 + step <= nt && cmp_row_q(T, h0 + step - 1, q, nk, f) == 0) { h0 += step; step <<= 1; }
-      const u64 top = h0 + step <= nt ? h0 + step : nt;
-      h0 = upper_bound_q(T, h0, top, q, nk, f);
-    }
+    u64 l0, h0;
+    warp_key_range(s, tr, b, q, active, nk, f, l0, h0);
     lo[b] = (u32)l0;
     hi[b] = (u32)h0;
   }
+  if (!active) return;
   bool have = false, exhausted = false;
   i64 wsum = 0;
   for (int it = 0; it < AGG_WALK; it++) {
@@ -1232,8 +1317,10 @@ static int32_t probe_chunk(Ctx* ctx, const Batch* delta, int nk, Batch* const* t
     // matched trace rows read once, delta rows read once, output rows written once
     ProfScope ps(ctx, KID_PROBE_FILL, (u64)total * (u64)(tb[0]->nl() - nk + 1) * 8 + nd * (u64)(delta->nl() + 1) * 8 +
                                           (u64)total * (u64)(Lo + 1) * 8);
-    k_probe_fill<<<(unsigned)((total + PF_TILE - 1) / PF_TILE), 256, 0, st>>>(delta->cols(), delta->w, nd, refs, nk, delta->nl() - nk, tb[0]->nl() - nk, lo,
-                                               cnt, ki, ex, total, proj ? 1 : 0, delta_is_left, pj, t.c, t.w);
+    const int spt = total >= PF_BIG_TILE_FROM ? 4 : 1;
+    const u64 tile = (u64)spt * PF_THREADS;
+    k_probe_fill<<<(unsigned)((total + tile - 1) / tile), PF_THREADS, 0, st>>>(delta->cols(), delta->w, nd, refs, nk, delta->nl() - nk, tb[0]->nl() - nk, lo,
+                                               cnt, ki, ex, total, spt, proj ? 1 : 0, delta_is_left, pj, t.c, t.w);
   }
   LAUNCH_COUNT(ctx);
   // the Batcher of join.rs:845-858: usually sort-free (ordered slots)

@@ -141,6 +141,8 @@ _SIGS = {
     "semijoin": [_P, _P, _P, _PP],
     "aggregate_delta": [_P, _P, _P, _P, C.c_int32, _PP],
     "aggregate_fold": [_P, _P, _P, _P, C.POINTER(CFold), _PP],
+    "upsert_commands": [_P, C.POINTER(CSchema), _PP, _P, C.c_uint64, C.c_uint64, C.c_int32, _PP],
+    "upsert_delta": [_P, _P, _P, _PP],
     "weigh": [_P, _P, C.POINTER(CExpr), C.c_int32, _PP],
     "weigh_fn": [_P, _P, C.POINTER(CRowFn), C.c_int32, _PP],
     "distinct_delta": [_P, _P, _P, _PP],
@@ -168,7 +170,7 @@ ROWFN_CALLS = {"batch_from_table_fn", "batch_from_upload_fn", "join_delta_trace_
                "map_index_fn", "batch_from_table_fanout", "batch_from_upload_fanout", "map_index_fanout"}
 # Operators added after that oracle: the CUDA library and the row-function oracle export them, the dbsp_proj oracle
 # does not.  `CApi.exports` tells a caller which of them a library has.
-LATER_CALLS = {"antijoin_delta", "aggregate_fold"}
+LATER_CALLS = {"antijoin_delta", "aggregate_fold", "upsert_commands", "upsert_delta"}
 
 
 class CApi:

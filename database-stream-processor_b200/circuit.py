@@ -19,7 +19,7 @@ import numpy as np
 
 from . import _capi as capi
 from .zset import (Backend, Batch, Expr, Fn, Pred, Proj, Schema, Spine, Src, acc, compile_fold, compile_fold_step, const, key,
-                   lval, rval)
+                   lval, rval, upsert_command_schema)
 
 
 class Max:  # operator/aggregate/max.rs:36-55
@@ -151,6 +151,112 @@ class TableHandle:
         return cur
 
 
+_M64 = (1 << 64) - 1
+
+
+class UpsertHandle:
+    """UpsertHandle (operator/input.rs:747-882): the commands of a set or map input table.  The commands buffered
+    between steps form the next step's; per key only the last one counts.  A key is an int (one key lane) or a tuple
+    of the key lanes, a map's value likewise for the value lanes.
+
+    A set's command is push(key, insert) with a bool; a map's is push(key, value), value None deleting the key.
+    For bulk loads, append_columns(cols, insert=None) takes host numpy columns and append_device(ptrs, n,
+    insert=None) resident device columns: the table's lanes (a delete's value lanes are ignored) and one flag per
+    command (None: every command inserts).  Appends keep their order within a step, whatever their kind."""
+
+    # A step's commands on worker r are numbered from r << SEQ_RANK_SHIFT: a key's commands are ordered by worker
+    # rank, then push order, and a worker may take up to 2^40 commands per step.
+    SEQ_RANK_SHIFT = 40
+
+    def __init__(self, circuit, schema: Schema, is_map: bool):
+        self.circuit, self.schema, self.is_map = circuit, schema, is_map
+        self.pending = []   # ("rows", [(lanes, insert)]) | ("host", cols, insert) | ("dev", ptrs, n, insert)
+
+    @staticmethod
+    def _lanes(x, n, what):
+        t = tuple(x) if isinstance(x, (tuple, list)) else (x,)
+        if len(t) != n or not all(isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_)) for v in t):
+            raise ValueError(f"UpsertHandle: {what} must be {n} integer lane(s), got {x!r}")
+        return t
+
+    def _command(self, key, value):
+        s = self.schema
+        k = self._lanes(key, s.nk, "a key")
+        if not self.is_map:
+            if not isinstance(value, (bool, np.bool_)):
+                raise ValueError(f"UpsertHandle: a set's command is (key, bool), got the value {value!r}")
+            return k, bool(value)
+        if value is None:
+            return k + (0,) * s.nv, False
+        return k + self._lanes(value, s.nv, "a value"), True
+
+    def _rows(self, rows):
+        if not rows:
+            return
+        if not self.pending or self.pending[-1][0] != "rows":
+            self.pending.append(("rows", []))
+        self.pending[-1][1].extend(rows)
+
+    def push(self, key, value):
+        """push (input.rs:802-815): one command."""
+        self._rows([self._command(key, value)])
+
+    def append(self, commands):
+        """append (input.rs:836-877): (key, value) commands in order; a malformed one raises before any is taken."""
+        self._rows([self._command(k, v) for k, v in commands])
+
+    def append_columns(self, cols, insert=None):
+        """Commands as host columns: the table's lanes, and one insert flag per command (None: all insert)."""
+        cols = [np.asarray(c) for c in cols]
+        n = self._check_columns(len(cols), [len(c) for c in cols], insert)
+        if n:
+            self.pending.append(("host", cols, insert))
+
+    def append_device(self, ptrs, n, insert=None):
+        """Commands as resident device columns (raw addresses of n u64 each) and an optional device array of n u8
+        insert flags."""
+        ptrs = list(ptrs)
+        self._check_columns(len(ptrs), [int(n)] * len(ptrs), None)
+        if int(n):
+            self.pending.append(("dev", ptrs, int(n), insert))
+
+    def _check_columns(self, n_cols, lens, insert):
+        s = self.schema
+        if n_cols != s.nl:
+            raise ValueError(f"UpsertHandle: the table has {s.nl} lanes, got {n_cols} columns")
+        if len(set(lens)) > 1:
+            raise ValueError(f"UpsertHandle: columns of different lengths {lens}")
+        n = lens[0]
+        if insert is not None and len(insert) != n:
+            raise ValueError(f"UpsertHandle: {len(insert)} insert flags for {n} commands")
+        return n
+
+    def clear_input(self):
+        """clear_input (input.rs:879-882): drop the commands buffered since the last step."""
+        self.pending = []
+
+    def _take(self) -> Batch:
+        """This step's commands as one command batch, in order."""
+        chunks, self.pending = self.pending, []
+        be, comm, s = self.circuit.be, self.circuit.comm, self.schema
+        seq = (comm.rank if comm is not None else 0) << self.SEQ_RANK_SHIFT
+        out = None
+        for c in chunks:
+            if c[0] == "rows":
+                arr = np.array([[int(x) & _M64 for x in r[0]] for r in c[1]], dtype=np.uint64).reshape(len(c[1]), s.nl)
+                b = be.upsert_commands(s, [arr[:, i] for i in range(s.nl)], [r[1] for r in c[1]], seq0=seq)
+                n = len(c[1])
+            elif c[0] == "host":
+                b = be.upsert_commands(s, c[1], c[2], seq0=seq)
+                n = len(c[1][0])
+            else:
+                b = be.upsert_commands(s, c[1], c[3], n=c[2], seq0=seq, on_device=True)
+                n = c[2]
+            seq += n
+            out = b if out is None else be.merge(out, b)
+        return out if out is not None else be.batch_empty(upsert_command_schema(s))
+
+
 class RootCircuit:
     """RootCircuit::build + CircuitHandle::step
     (circuit_builder.rs:1403-1433, 3658-3663)."""
@@ -174,6 +280,38 @@ class RootCircuit:
         return Stream(self, node, schema), h
 
     add_input_indexed_zset = add_input_zset
+
+    def add_input_set(self, schema: Schema):
+        """add_input_set (operator/input.rs:168-245): an OrdZSet of the schema's lanes (all of them key lanes) fed by
+        insert / delete commands with set semantics: inserting a present row and deleting an absent one do nothing.
+        Returns (stream, UpsertHandle)."""
+        return self._add_upsert(Schema(schema.lanes), is_map=False)
+
+    def add_input_map(self, schema: Schema):
+        """add_input_map (operator/input.rs:247-328): an indexed Z-set with the schema's key and value lanes (at
+        least one of each) fed by upserts: a key's new value retracts its old one, a delete retracts it.  Returns
+        (stream, UpsertHandle)."""
+        if schema.nk == 0 or schema.nv == 0:
+            raise ValueError(f"add_input_map: a map has key lanes and value lanes, got {schema}")
+        return self._add_upsert(schema, is_map=True)
+
+    def _add_upsert(self, schema: Schema, is_map: bool):
+        """add_upsert (input.rs:128-166) + Upsert (operator/upsert.rs): the step's command batch, sharded by key, is
+        applied to the table's trace, which the stream owns (`stream.table_trace`)."""
+        be = self.be
+        be.upsert_commands(schema, [np.zeros(0, np.uint64)] * schema.nl)   # the library refuses a bad table now
+        h = UpsertHandle(self, schema, is_map)
+        cmds = Stream(self, Node(self, [], h._take, "upsert_commands"), upsert_command_schema(schema)).shard()
+        table = Spine(be, schema)
+
+        def fn(c: Batch):
+            out = be.upsert_delta(c, table)
+            table.insert(out)
+            return out
+
+        out = cmds._unary(fn, "upsert", schema, True)
+        out.table_trace = table
+        return out, h
 
     def add_input_table(self, n_cols: int):
         h = TableHandle()

@@ -1396,6 +1396,32 @@ int32_t dbsp_aggregate_fold(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine
   NOT_NULL(out_tr, "out_trace");
   REFUSE(dv::valid_fold(B(d)->s, in_tr->s, out_tr->s, fold));
   OUT1(op_aggregate_fold(ctx, B(d), in_tr, out_tr, fold, &o__)) }
+int32_t dbsp_upsert_commands(dbsp_ctx* ctx, const dbsp_schema* table, const uint64_t* const* cols,
+                             const uint8_t* insert, uint64_t n, uint64_t seq0, int32_t on_device,
+                             dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_upsert(table, n, seq0));
+  const int L = table->n_key_lanes + table->n_val_lanes;
+  REFUSE(valid_cols(WHAT, cols, L, n));
+  ROWS32(n);
+  BufP hold, ihold;
+  Cols dc;
+  const i64* dw;
+  TRY(stage_columns(ctx, cols, L, nullptr, n, on_device, &hold, &dc, &dw));
+  const uint8_t* dins = insert;
+  if (insert && !on_device && n) {
+    TRY(dev_alloc(ctx, (size_t)n, &ihold));
+    CUDA_TRY(cudaMemcpyAsync(ihold->p, insert, n, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->h2d_bytes += n;
+    dins = (const uint8_t*)ihold->p;
+  }
+  OUT1(op_upsert_commands(ctx, *table, dc, dins, n, seq0, &o__)) }
+int32_t dbsp_upsert_delta(dbsp_ctx* ctx, const dbsp_batch* cmds, const dbsp_spine* table, dbsp_batch** out) { ENTER(ctx);
+  NOT_NULL(out, "out");
+  NOT_NULL(cmds, "cmds");
+  NOT_NULL(table, "table");
+  REFUSE(dv::valid_upsert(B(cmds)->s, table->s));
+  OUT1(op_upsert_delta(ctx, B(cmds), table, &o__)) }
 int32_t dbsp_weigh(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_expr* f, int32_t mode, dbsp_batch** out) { ENTER(ctx);
   NOT_NULL(out, "out");
   NOT_NULL(b, "batch");

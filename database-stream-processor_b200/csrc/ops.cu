@@ -745,6 +745,32 @@ __global__ void k_key_heads(Cols C, u64 n, int nk, u32* flags) {
   flags[i] = head ? 1u : 0u;
 }
 
+// The commands of a set / map input (operator/input.rs:128-166): key lanes, the command word ((seq0 + i) << 1 |
+// insert), value lanes (0 for a delete), weight 1.  insert == nullptr: every command inserts.
+__global__ void k_upsert_cmds(Cols in, int nk, int nv, const uint8_t* insert, u64 n, u64 seq0, MCols out, i64* out_w) {
+  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const bool ins = insert == nullptr || insert[i] != 0;
+  for (int l = 0; l < nk; l++) out.c[l][i] = in.c[l][i];
+  out.c[nk][i] = ((seq0 + i) << 1) | (ins ? 1u : 0u);
+  for (int l = 0; l < nv; l++) out.c[nk + 1 + l][i] = ins ? in.c[nk + l][i] : 0;
+  out_w[i] = 1;
+}
+
+// Over commands sorted by (key, command word): each key's last command (input.rs:147-160 keeps it), and among those
+// the inserts (command bit 1).  last[n] = ins[n] = 0 for the ordered compaction.
+__global__ void k_upsert_last(Cols C, u64 n, int nk, u32* last, u32* ins) {
+  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > n) return;
+  if (i == n) { last[n] = 0; ins[n] = 0; return; }
+  bool is_last = i == n - 1;
+  if (!is_last)
+    for (int l = 0; l < nk; l++)
+      if (C.c[l][i] != C.c[l][i + 1]) { is_last = true; break; }
+  last[i] = is_last ? 1u : 0u;
+  ins[i] = (is_last && (C.c[nk][i] & 1)) ? 1u : 0u;
+}
+
 // ordered compaction: out[pos[i]] = row i for keep[i] != 0
 __global__ void k_scatter(Cols in, int L, const i64* w, const u32* keep, const u32* pos, u64 n, MCols out, i64* out_w) {
   u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1539,6 +1565,54 @@ int32_t op_aggregate_fold(Ctx* ctx, const Batch* delta, const Spine* in_tr, cons
   batch_unref(G);
   if (rc) { batch_unref(keys); return rc; }
   return upsert_keys(ctx, keys, N, out_tr, out);
+}
+
+// The command batch of dbsp_upsert_commands: k_upsert_cmds over the (staged) columns, then the consolidation, whose
+// order (key, command word) is add_upsert's stable sort by key (input.rs:141-145).  Command words are unique, so no
+// two rows are summed.
+int32_t op_upsert_commands(Ctx* ctx, const dbsp_schema& table, const Cols& in, const uint8_t* insert, u64 n, u64 seq0,
+                           Batch** out) {
+  const dbsp_schema cs = dbsp_validate::upsert_command_schema(table);
+  if (n == 0) { *out = batch_new_empty(ctx, cs); return DBSP_OK; }
+  const int nk = table.n_key_lanes, nv = table.n_val_lanes;
+  TmpRows t;
+  TRY(tmp_alloc(ctx, nk + 1 + nv, n, &t));
+  k_upsert_cmds<<<blocks(n), TB, 0, ctx->stream>>>(in, nk, nv, insert, n, seq0, t.c, t.w);
+  LAUNCH_COUNT(ctx);
+  return consolidate_rows(ctx, cs, t.cc(), t.w, n, &t.buf, out);
+}
+
+// Upsert::eval (operator/upsert.rs:161-208) after add_upsert's last-command-per-key step (input.rs:147-160): the
+// affected keys and the +1 rows of the inserting ones by ordered compaction (both stay in key order), then the probe
+// of the table's trace, negate and merge that aggregates share.
+int32_t op_upsert_delta(Ctx* ctx, const Batch* cmds, const Spine* table, Batch** out) {
+  const dbsp_schema& ts = table->s;
+  const int nk = ts.n_key_lanes, nv = ts.n_val_lanes;
+  const u64 n = cmds->n;
+  if (n == 0) { *out = batch_new_empty(ctx, ts); return DBSP_OK; }
+  ROWS32(n, "upsert_delta");
+  BufP fb;
+  TRY(dev_alloc(ctx, (size_t)(n + 1) * 4 * 2, &fb));
+  u32* last = (u32*)fb->p;
+  u32* ins = last + (n + 1);
+  {
+    // the key lanes and the command lane read once, the two flag arrays written once
+    ProfScope ps(ctx, KID_UPSERT, n * (u64)(nk + 1) * 8 + (n + 1) * 8);
+    k_upsert_last<<<blocks(n + 1), TB, 0, ctx->stream>>>(cmds->cols(), n, nk, last, ins);
+  }
+  LAUNCH_COUNT(ctx);
+  dbsp_schema ks;
+  memset(&ks, 0, sizeof(ks));
+  ks.n_key_lanes = nk;
+  for (int l = 0; l < nk; l++) ks.lane_types[l] = ts.lane_types[l];
+  Batch* keys = nullptr;
+  TRY(compact_ordered(ctx, ks, cmds->cols(), cmds->w, last, n, &keys));
+  MCols vals;   // read only: new_values gathers them with the key lanes
+  for (int l = 0; l < MAXL; l++) vals.c[l] = l < nv ? const_cast<u64*>(cmds->col[nk + 1 + l]) : nullptr;
+  Batch* N = nullptr;
+  const int32_t rc = new_values(ctx, ts, cmds->col, vals, ins, n, &N);
+  if (rc) { batch_unref(keys); return rc; }
+  return upsert_keys(ctx, keys, N, table, out);
 }
 
 int32_t op_neg(Ctx* ctx, const Batch* a, Batch** out) {

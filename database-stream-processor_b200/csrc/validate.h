@@ -234,7 +234,50 @@ inline std::string valid_antijoin(const dbsp_schema& delta, const dbsp_schema& t
   return "";
 }
 
-// ---- snapshot files (dbsp_spine_save / dbsp_spine_load) ---------------------------------------------------------
+// ---- set and map input tables (dbsp_upsert_commands / dbsp_upsert_delta) ----------------------------------------
+// The command batch of a table: its key lanes as keys, then one u64 command lane and its value lanes as values.
+inline dbsp_schema upsert_command_schema(const dbsp_schema& t) {
+  dbsp_schema c;
+  memset(&c, 0, sizeof(c));
+  c.n_key_lanes = t.n_key_lanes;
+  c.n_val_lanes = (uint8_t)(t.n_val_lanes + 1);
+  for (int l = 0; l < t.n_key_lanes; l++) c.lane_types[l] = t.lane_types[l];
+  c.lane_types[t.n_key_lanes] = DBSP_U64;
+  for (int l = 0; l < t.n_val_lanes; l++) c.lane_types[t.n_key_lanes + 1 + l] = t.lane_types[t.n_key_lanes + l];
+  return c;
+}
+// A table has at least one key lane (an upsert replaces a key's value) and at most 7 lanes (the command lane takes the
+// 8th of the command batch).
+inline std::string valid_upsert_table(const dbsp_schema* t, const std::string& what) {
+  std::string m = valid_schema(t, what, "table");
+  if (!m.empty()) return m;
+  if (t->n_key_lanes == 0) return what + ": table has no key lanes; a command replaces a key's row";
+  const int L = t->n_key_lanes + t->n_val_lanes;
+  if (L > DBSP_MAX_LANES - 1)
+    return what + ": table has " + num(L) + " lanes; the command lane takes the 8th, so a table has at most 7";
+  return "";
+}
+// upsert_commands: a valid table, and sequence numbers seq0 .. seq0 + n - 1 that fit 63 bits (the command word is
+// the sequence number shifted left by one, the insert bit below it).
+inline std::string valid_upsert(const dbsp_schema* table, uint64_t n, uint64_t seq0) {
+  const std::string what = "upsert_commands";
+  std::string m = valid_upsert_table(table, what);
+  if (!m.empty()) return m;
+  if (seq0 > (1ull << 63) || n > (1ull << 63) - seq0)
+    return what + ": seq0 + n = " + num(seq0) + " + " + num(n) + " exceeds 2^63; a command's sequence number has 63 bits";
+  return "";
+}
+// upsert_delta: a valid table, and a command batch with the schema upsert_commands gives for it.
+inline std::string valid_upsert(const dbsp_schema& cmds, const dbsp_schema& table) {
+  const std::string what = "upsert_delta";
+  std::string m = valid_upsert_table(&table, what);
+  if (!m.empty()) return m;
+  if (!same_schema(cmds, upsert_command_schema(table)))
+    return what + ": cmds must have the table's key lanes, then a u64 command lane and the table's value lanes";
+  return "";
+}
+
+// ---- snapshot files (dbsp_spine_save / dbsp_spine_load)---------------------------------------------------------
 // header: magic, schema, {has key bound, has value bound, effort, layer count}, key bound, value bound
 inline std::string valid_snapshot_header(const dbsp_schema& s, const uint64_t hdr[4]) {
   std::string m = valid_schema(&s, "spine_load", "file schema");

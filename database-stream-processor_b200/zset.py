@@ -61,6 +61,11 @@ class Schema:
         return Schema(self.lanes[:nk], self.lanes[nk:])
 
 
+def upsert_command_schema(table: Schema) -> Schema:
+    """The command batch of a set / map input: the table's key lanes, then a u64 command lane and its value lanes."""
+    return Schema(table.key, "u" + table.val)
+
+
 # ---- declarative row expressions (stand in for the Rust closures) --------
 # A closure whose lanes are single operations over two sources and whose filter is at most MAX_PREDS comparisons of
 # two sources compiles to a `dbsp_proj`.  Anything else (nested arithmetic, %, abs, min/max, bitwise ops, shifts,
@@ -965,6 +970,29 @@ class Backend:
         out = self._out()
         self.api.call("aggregate_fold", self.ctx, delta.h, in_trace.h, out_trace.h, C.byref(fold._c), C.byref(out))
         return Batch(self, out.value, out_trace.schema)
+
+    def upsert_commands(self, table: Schema, cols: Sequence, insert=None, n=None, seq0: int = 0, on_device=False) -> Batch:
+        """The commands of a set / map input as a batch (dbsp_upsert_commands): command i is row i of `cols` (the
+        table's lanes) with the sequence number seq0 + i; `insert` (one flag per command, None: all insert) tells
+        inserts from deletes.  Host inputs are numpy arrays; device inputs are raw addresses (on_device=True)."""
+        if not on_device:
+            cols = [as_u64(c) for c in cols]
+            n = len(cols[0]) if cols else 0
+            if insert is not None:
+                insert = np.ascontiguousarray(np.asarray(insert) != 0, dtype=np.uint8)
+            iptr = insert.ctypes.data if insert is not None else None
+        else:
+            iptr = insert
+        out = self._out()
+        self.api.call("upsert_commands", self.ctx, C.byref(table.c()), col_ptrs(cols), iptr, n, seq0, int(on_device),
+                      C.byref(out))
+        return Batch(self, out.value, upsert_command_schema(table))
+
+    def upsert_delta(self, cmds: Batch, table: Spine) -> Batch:
+        """Upsert::eval of a command batch against the table's trace: the table's change (dbsp_upsert_delta)."""
+        out = self._out()
+        self.api.call("upsert_delta", self.ctx, cmds.h, table.h, C.byref(out))
+        return Batch(self, out.value, table.schema)
 
     def weigh(self, b: Batch, f, mode: int) -> Batch:
         """f: a value of the key / value lanes, or a one-lane Proj whose filter drops rows."""

@@ -497,6 +497,34 @@ int32_t dbsp_aggregate_fold(dbsp_ctx* ctx, const dbsp_batch* delta,
                             const dbsp_spine* in_trace,
                             const dbsp_spine* out_trace, const dbsp_fold* fold,
                             dbsp_batch** out);
+/* The commands of a set or map input table (operator/input.rs:128-328,
+ * add_input_set / add_input_map) as a batch.  `table` is the table's schema:
+ * at least one key lane and at most 7 lanes in all (a set has key lanes
+ * only).  The batch has the table's key lanes as its keys, then as values one
+ * u64 command lane and the table's value lanes.  Command i (0 <= i < n) is
+ * the row cols[0..nk+nv)[i] with the command word
+ *   ((seq0 + i) << 1) | (insert[i] != 0)
+ * and weight 1; a delete's value lanes are written as 0.  insert == NULL:
+ * every command inserts.  seq0 + n is at most 2^63 (a sequence number has 63
+ * bits).  on_device as in dbsp_batch_from_tuples (cols and insert).  The rows are
+ * consolidated, so they come out ordered by (key, command word): a stable sort
+ * by key of the commands in sequence order (input.rs:141-145).  Batches of
+ * commands with distinct sequence numbers merge (and shard) into one batch in
+ * the same order. */
+int32_t dbsp_upsert_commands(dbsp_ctx* ctx, const dbsp_schema* table,
+                             const uint64_t* const* cols,
+                             const uint8_t* insert, uint64_t n, uint64_t seq0,
+                             int32_t on_device, dbsp_batch** out);
+/* Upsert::eval (operator/upsert.rs:155-208) of a command batch against the
+ * table's trace: per key with a command, only the last command counts
+ * (input.rs:147-160); the key's current rows in `table` (weights summed over
+ * its batches, zero sums skipped) are retracted with their negated weights,
+ * and (key, v) is inserted with weight +1 if that command inserts.  The
+ * result is consolidated, with the table's schema; the caller inserts it into
+ * `table` (upsert.rs:69-107).  `cmds` has the schema dbsp_upsert_commands
+ * gives for the table; its weights are not read. */
+int32_t dbsp_upsert_delta(dbsp_ctx* ctx, const dbsp_batch* cmds,
+                          const dbsp_spine* table, dbsp_batch** out);
 /* weigh (aggregate/mod.rs:297-323). `f` gives f(k,v) (SRC_KEY/SRC_LVAL).
  * `mode` is a dbsp_weigh_mode; WEIGH_AVG adds a key lane (at most 7 before). */
 int32_t dbsp_weigh(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_expr* f,

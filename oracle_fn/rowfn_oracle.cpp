@@ -1,9 +1,9 @@
 // rowfn_oracle.cpp — the CPU oracle with row functions (dbsp_rowfn, include/dbsp_b200.h): the whole oracle of
-// oracle/dbsp_oracle.cpp, unchanged, plus the `_fn` and `_fanout` entry points, dbsp_antijoin_delta and
-// dbsp_aggregate_fold, in one translation unit so that they build on its
-// batches, traces, consolidation and error text.  The oracle's own library stays the checker of every `dbsp_proj`
-// test; this one (libdbsp_oracle_fn.so, test infrastructure like it, never linked into the product) is the checker
-// of the row-function, antijoin and fold tests.  The interpreter below is written apart from the CUDA library's; validate.h is shared,
+// oracle/dbsp_oracle.cpp, unchanged, plus the `_fn` and `_fanout` entry points, dbsp_antijoin_delta,
+// dbsp_aggregate_fold and the set / map input calls (dbsp_upsert_commands, dbsp_upsert_delta), in one translation unit
+// so that they build on its batches, traces, consolidation and error text.  The oracle's own library stays the checker
+// of every `dbsp_proj` test; this one (libdbsp_oracle_fn.so, test infrastructure like it, never linked into the
+// product) is the checker of the row-function, antijoin, fold and upsert tests.  The interpreter below is written apart from the CUDA library's; validate.h is shared,
 // so both libraries refuse the same programs with the same texts.
 #include "../oracle/dbsp_oracle.cpp"
 
@@ -291,6 +291,61 @@ int32_t orc_aggregate_fold(orc_ctx* c, const orc_batch* delta, const orc_spine* 
       has_new = st[nov] != 0;
     }
     upsert_key(bld, out_tr->s, key, st, has_new);
+  }
+  *out = wrap(bld.done());
+  return DBSP_OK;
+}
+
+// The commands of a set / map input as a batch: (key, command word, value) rows, a delete's values 0, consolidated.
+int32_t orc_upsert_commands(orc_ctx* c, const dbsp_schema* table, const u64* const* cols, const uint8_t* insert, u64 n,
+                            u64 seq0, int32_t, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  REFUSE(dv::valid_upsert(table, n, seq0));
+  const int nk = table->n_key_lanes, nv = table->n_val_lanes;
+  REFUSE(valid_cols(WHAT, cols, nk + nv, n));
+  ROWS32(n);
+  Tuples t(dv::upsert_command_schema(*table));
+  u64 row[MAXL];
+  for (u64 i = 0; i < n; i++) {
+    const bool ins = insert == nullptr || insert[i] != 0;
+    for (int l = 0; l < nk; l++) row[l] = cols[l][i];
+    row[nk] = ((seq0 + i) << 1) | (ins ? 1 : 0);
+    for (int l = 0; l < nv; l++) row[nk + 1 + l] = ins ? cols[nk + l][i] : 0;
+    t.push(row, 1);
+  }
+  *out = wrap(t.build());
+  return DBSP_OK;
+}
+
+// add_upsert (operator/input.rs:141-160) and Upsert::eval (operator/upsert.rs:161-208), as they read: the commands in
+// sequence order, stable-sorted by key, the last command of each key kept, then per key a seek into the table's trace
+// that retracts its current values and inserts the new one.  Written apart from the CUDA library's flags and
+// compactions.
+int32_t orc_upsert_delta(orc_ctx* c, const orc_batch* cmds, const orc_spine* table, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  NOT_NULL(out, "out");
+  NOT_NULL(cmds, "cmds");
+  NOT_NULL(table, "table");
+  REFUSE(dv::valid_upsert(cmds->p->s, table->s.s));
+  const Batch& C = *cmds->p;
+  const dbsp_schema& ts = table->s.s;
+  // the commands: row j of the batch, its key at kof[j], its command word in value lane 0, its values after it
+  std::vector<uint32_t> kof(C.len());
+  for (size_t k = 0; k < C.K.n; k++)
+    for (size_t j = C.offs[k]; j < C.offs[k + 1]; j++) kof[j] = (uint32_t)k;
+  const std::vector<u64>& word = C.V.c[0];
+  std::vector<size_t> v(C.len());
+  for (size_t j = 0; j < v.size(); j++) v[j] = j;
+  std::sort(v.begin(), v.end(), [&](size_t a, size_t b) { return word[a] < word[b]; });   // arrival order
+  std::stable_sort(v.begin(), v.end(), [&](size_t a, size_t b) { return cmp_rows(C.K, kof[a], C.K, kof[b]) < 0; });
+  Builder bld(ts);
+  u64 key[MAXL], cv[MAXL];
+  for (size_t i = 0; i < v.size(); i++) {
+    if (i + 1 < v.size() && kof[v[i]] == kof[v[i + 1]]) continue;   // a later command of the key follows
+    C.K.get(kof[v[i]], key);
+    C.V.get(v[i], cv);
+    upsert_key(bld, table->s, key, cv + 1, (cv[0] & 1) != 0);
   }
   *out = wrap(bld.done());
   return DBSP_OK;

@@ -20,52 +20,30 @@ struct dbsp_batcher;
 
 static inline Batch* B(const dbsp_batch* b) { return (Batch*)b; }
 static inline dbsp_batch* H(Batch* b) { return (dbsp_batch*)b; }
+// a handle's schema as the checks of validate.h take it: NULL for a NULL handle
+static inline const dbsp_schema* S(const dbsp_batch* b) { return b ? &B(b)->s : nullptr; }
+static inline const dbsp_schema* S(const dbsp_spine* s) { return s ? &s->s : nullptr; }
 
+// The error contract of include/dbsp_b200.h: every argument is checked on the host, by the call's check in
+// validate.h, before the call allocates, copies or launches anything.  WHAT is the call's name without the prefix.
+namespace dv = dbsp_validate;
+#define WHAT (__func__ + 5)
+#define REFUSE(check)                                          \
+  do {                                                         \
+    const dv::Refusal r__ = (check);                           \
+    if (r__) { set_error(r__.text); return r__.status; }       \
+  } while (0)
+#define NOT_NULL(p, name) REFUSE(dv::not_null(p, WHAT, name))
 // every entry point makes the context's device current: a host may drive several contexts (GPUs) from one
 // process, one per worker thread (INTEGRATION.md §3)
-#define CHECK_ARG(c, msg)                 \
-  do {                                    \
-    if (!(c)) { set_error(msg); return DBSP_ERR_INVALID; } \
-  } while (0)
-// The error contract of include/dbsp_b200.h: every argument is checked on the host before the call allocates, copies
-// or launches anything.  WHAT is the call's name without the prefix; the texts name the call and the argument.
-#define WHAT (__func__ + 5)
-#define NOT_NULL(p, name) CHECK_ARG((p) != nullptr, std::string(WHAT) + ": " name " is NULL")
-#define REFUSE(text)                                                  \
-  do {                                                                \
-    const std::string m__ = (text);                                   \
-    if (!m__.empty()) { set_error(m__); return DBSP_ERR_INVALID; }   \
-  } while (0)
 #define ENTER(c)        \
   NOT_NULL(c, "ctx");   \
   CUDA_TRY(cudaSetDevice((c)->device))
-namespace dv = dbsp_validate;
-// Row indices are 32-bit on the device: a batch of 2^32-1 or more rows is refused, never wrapped.
-#define ROWS32(n)                                                                                \
-  do {                                                                                           \
-    if ((u64)(n) >= 0xffffffffull) {                                                             \
-      set_error(std::string(WHAT) + ": n = " + std::to_string(n) + ": 2^32-1 or more rows in one batch; split the batch"); \
-      return DBSP_ERR_UNSUPPORTED;                                                               \
-    }                                                                                            \
-  } while (0)
-// a fan-out of n rows into n * n_out rows before consolidation: the same 32-bit bound, from the sizes alone
-#define FANOUT_ROWS(n, n_out)                                                                    \
-  do {                                                                                           \
-    const std::string m__ = dv::valid_fanout_rows((n), (n_out), WHAT);                           \
-    if (!m__.empty()) { set_error(m__); return DBSP_ERR_UNSUPPORTED; }                          \
-  } while (0)
 static RowFnFanout fanout_of(const dbsp_rowfn& fn, uint32_t n_out) {
   RowFnFanout f;
   static_cast<dbsp_rowfn&>(f) = fn;
   f.n_out = n_out;
   return f;
-}
-// host columns of a table or batch: the array and, when there are rows, each column the call reads
-static std::string valid_cols(const char* what, const u64* const* cols, int ncols, u64 n, unsigned mask = ~0u) {
-  if (!cols) return std::string(what) + ": cols is NULL";
-  for (int l = 0; n && l < ncols; l++)
-    if (((mask >> l) & 1) && !cols[l]) return std::string(what) + ": cols[" + std::to_string(l) + "] is NULL";
-  return "";
 }
 
 // Stage host columns on the device (stream-ordered).  Host memory may be
@@ -382,8 +360,7 @@ extern "C" {
 const char* dbsp_last_error(void) { return get_error(); }
 
 int32_t dbsp_ctx_create(int32_t device, dbsp_ctx** out) {
-  NOT_NULL(out, "out");
-  CHECK_ARG(device >= 0, "ctx_create: device is negative");
+  REFUSE(dv::check_ctx_create(out, device));
   int count = 0;
   cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess || count == 0 || device >= count) {
@@ -471,7 +448,7 @@ int32_t dbsp_ctx_sync_stats(dbsp_ctx* c, uint64_t* n_waits, double* wait_us, int
 void* dbsp_ctx_stream(dbsp_ctx* c) { return c ? (void*)c->stream : nullptr; }
 
 int32_t dbsp_ctx_profile(dbsp_ctx* c, int32_t enable) { ENTER(c);
-  CHECK_ARG(enable >= 0 && enable <= 2, "ctx_profile: enable must be 0, 1 or 2");
+  REFUSE(dv::check_ctx_profile(enable));
   if (enable == 2) { c->prof_on = false; return DBSP_OK; }   // pause: keep what was collected, record nothing more
   CUDA_TRY(cudaStreamSynchronize(c->stream));
   for (auto& r : c->prof) { c->ev_pool.push_back(r.a); c->ev_pool.push_back(r.b); }
@@ -500,11 +477,8 @@ int32_t dbsp_ctx_profile_read(dbsp_ctx* c, int32_t id, char* name32, uint64_t* l
 
 int32_t dbsp_batch_from_tuples(dbsp_ctx* ctx, const dbsp_schema* s, const uint64_t* const* cols, const int64_t* w,
                                uint64_t n, int32_t on_device, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_schema(s, WHAT));
+  REFUSE(dv::check_tuples(WHAT, out, s, cols, w, n, false));
   int L = s->n_key_lanes + s->n_val_lanes;
-  REFUSE(valid_cols(WHAT, cols, L, n));
-  ROWS32(n);
   BufP hold;
   Cols dc;
   const i64* dw;
@@ -517,11 +491,7 @@ int32_t dbsp_batch_from_tuples(dbsp_ctx* ctx, const dbsp_schema* s, const uint64
 
 int32_t dbsp_batch_from_table(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n_cols, const int64_t* w, uint64_t n,
                               int32_t on_device, const dbsp_proj* proj, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "batch_from_table: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
-  REFUSE(dv::valid_proj(proj, (int)n_cols, (int)n_cols, (int)n_cols, WHAT));
-  REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, dv::proj_table_mask(*proj)));
-  ROWS32(n);
+  REFUSE(dv::check_table(WHAT, out, cols, n_cols, n, proj));
   BufP hold;
   Cols dc;
   const i64* dw;
@@ -533,11 +503,7 @@ int32_t dbsp_batch_from_table(dbsp_ctx* ctx, const uint64_t* const* cols, uint32
 }
 int32_t dbsp_batch_from_table_fn(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n_cols, const int64_t* w,
                                  uint64_t n, int32_t on_device, const dbsp_rowfn* fn, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "batch_from_table_fn: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
-  REFUSE(dv::valid_rowfn(fn, (int)n_cols, (int)n_cols, (int)n_cols, WHAT));
-  REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, dv::rowfn_table_mask(*fn)));
-  ROWS32(n);
+  REFUSE(dv::check_table(WHAT, out, cols, n_cols, n, fn));
   BufP hold;
   Cols dc;
   const i64* dw;
@@ -551,13 +517,7 @@ int32_t dbsp_batch_from_table_fn(dbsp_ctx* ctx, const uint64_t* const* cols, uin
 int32_t dbsp_batch_from_table_fanout(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n_cols, const int64_t* w,
                                      uint64_t n, int32_t on_device, const dbsp_rowfn* fn, uint32_t n_out,
                                      dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "batch_from_table_fanout: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
-  REFUSE(dv::valid_fanout(n_out, WHAT));
-  REFUSE(dv::valid_rowfn(fn, (int)n_cols, (int)n_cols, (int)n_cols, WHAT, dv::SRC_BIT_FANOUT));
-  REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, dv::rowfn_table_mask(*fn)));
-  ROWS32(n);
-  FANOUT_ROWS(n, n_out);
+  REFUSE(dv::check_table(WHAT, out, cols, n_cols, n, fn, n_out));
   BufP hold;
   Cols dc;
   const i64* dw;
@@ -579,25 +539,18 @@ struct dbsp_upload {
   cudaEvent_t done;
 };
 
-uint32_t dbsp_proj_table_mask(const dbsp_proj* proj) {
-  if (!dv::valid_proj(proj, MAXL, MAXL, MAXL, "proj_table_mask").empty()) return 0;
-  return dv::proj_table_mask(*proj);
+static dv::Upload upload_of(const dbsp_upload* u, const Ctx* ctx) {
+  if (!u) return dv::Upload{false, false, 0, 0, 0};
+  return dv::Upload{true, u->ctx == ctx, u->n_cols, u->col_mask, u->n};
 }
-uint32_t dbsp_rowfn_table_mask(const dbsp_rowfn* fn) {
-  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "rowfn_table_mask").empty()) return 0;
-  return dv::rowfn_table_mask(*fn);
-}
-uint32_t dbsp_fanout_table_mask(const dbsp_rowfn* fn) {
-  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "fanout_table_mask", dv::SRC_BIT_FANOUT).empty()) return 0;
-  return dv::rowfn_table_mask(*fn);
-}
+
+uint32_t dbsp_proj_table_mask(const dbsp_proj* proj) { return dv::checked_table_mask(proj, WHAT); }
+uint32_t dbsp_rowfn_table_mask(const dbsp_rowfn* fn) { return dv::checked_table_mask(fn, WHAT); }
+uint32_t dbsp_fanout_table_mask(const dbsp_rowfn* fn) { return dv::checked_table_mask(fn, WHAT, dv::SRC_BIT_FANOUT); }
 
 int32_t dbsp_upload_begin(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n_cols, uint32_t col_mask,
                           const int64_t* w, uint64_t n, dbsp_upload** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "upload_begin: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
-  REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, col_mask));
-  ROWS32(n);
+  REFUSE(dv::check_upload_begin(out, cols, n_cols, col_mask, n));
   dbsp_upload* u = new dbsp_upload();
   u->ctx = ctx;
   u->n = n;
@@ -648,14 +601,7 @@ int32_t dbsp_upload_begin(dbsp_ctx* ctx, const uint64_t* const* cols, uint32_t n
 }
 
 int32_t dbsp_batch_from_upload(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_proj* proj, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(u, "upload");
-  CHECK_ARG(u->ctx == ctx, "batch_from_upload: upload belongs to another context");
-  REFUSE(dv::valid_proj(proj, u->n_cols, u->n_cols, u->n_cols, WHAT));
-  {
-    const unsigned missing = dv::proj_table_mask(*proj) & ~u->col_mask;
-    CHECK_ARG(missing == 0, "batch_from_upload: proj reads column " + std::to_string(__builtin_ctz(missing | 0x100u)) + ", which col_mask left out of the upload");
-  }
+  REFUSE(dv::check_upload(WHAT, out, upload_of(u, ctx), proj));
   CUDA_TRY(cudaStreamWaitEvent(ctx->stream, u->done, 0));   // compute stream waits for the copy
   Batch* b = nullptr;
   TRY(project_and_consolidate(ctx, u->dc, 0, u->n_cols, u->dw, u->n, *proj, &b));
@@ -663,14 +609,7 @@ int32_t dbsp_batch_from_upload(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_proj* p
   return DBSP_OK;
 }
 int32_t dbsp_batch_from_upload_fn(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_rowfn* fn, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(u, "upload");
-  CHECK_ARG(u->ctx == ctx, "batch_from_upload_fn: upload belongs to another context");
-  REFUSE(dv::valid_rowfn(fn, u->n_cols, u->n_cols, u->n_cols, WHAT));
-  {
-    const unsigned missing = dv::rowfn_table_mask(*fn) & ~u->col_mask;
-    CHECK_ARG(missing == 0, "batch_from_upload_fn: fn reads column " + std::to_string(__builtin_ctz(missing | 0x100u)) + ", which col_mask left out of the upload");
-  }
+  REFUSE(dv::check_upload(WHAT, out, upload_of(u, ctx), fn));
   CUDA_TRY(cudaStreamWaitEvent(ctx->stream, u->done, 0));   // compute stream waits for the copy
   Batch* b = nullptr;
   TRY(project_and_consolidate(ctx, u->dc, 0, u->n_cols, u->dw, u->n, *fn, &b));
@@ -680,16 +619,7 @@ int32_t dbsp_batch_from_upload_fn(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_rowf
 
 int32_t dbsp_batch_from_upload_fanout(dbsp_ctx* ctx, dbsp_upload* u, const dbsp_rowfn* fn, uint32_t n_out,
                                       dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(u, "upload");
-  CHECK_ARG(u->ctx == ctx, "batch_from_upload_fanout: upload belongs to another context");
-  REFUSE(dv::valid_fanout(n_out, WHAT));
-  REFUSE(dv::valid_rowfn(fn, u->n_cols, u->n_cols, u->n_cols, WHAT, dv::SRC_BIT_FANOUT));
-  {
-    const unsigned missing = dv::rowfn_table_mask(*fn) & ~u->col_mask;
-    CHECK_ARG(missing == 0, "batch_from_upload_fanout: fn reads column " + std::to_string(__builtin_ctz(missing | 0x100u)) + ", which col_mask left out of the upload");
-  }
-  FANOUT_ROWS(u->n, n_out);
+  REFUSE(dv::check_upload(WHAT, out, upload_of(u, ctx), fn, n_out));
   CUDA_TRY(cudaStreamWaitEvent(ctx->stream, u->done, 0));   // compute stream waits for the copy
   Batch* b = nullptr;
   TRY(project_and_consolidate(ctx, u->dc, 0, u->n_cols, u->dw, u->n, fanout_of(*fn, n_out), &b));
@@ -709,12 +639,8 @@ int32_t dbsp_upload_free(dbsp_upload* u) {
 
 int32_t dbsp_batch_from_sorted(dbsp_ctx* ctx, const dbsp_schema* s, const uint64_t* const* cols, const int64_t* w,
                                uint64_t n, int32_t on_device, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_schema(s, WHAT));
+  REFUSE(dv::check_tuples(WHAT, out, s, cols, w, n, true));
   int L = s->n_key_lanes + s->n_val_lanes;
-  REFUSE(valid_cols(WHAT, cols, L, n));
-  CHECK_ARG(n == 0 || w != nullptr, "batch_from_sorted: weights is NULL (consolidated rows carry their weights)");
-  ROWS32(n);
   if (n == 0) { *out = H(batch_new_empty(ctx, *s)); return DBSP_OK; }
   Batch* b;
   MCols oc;
@@ -753,8 +679,7 @@ static int32_t batcher_enqueue(Ctx* ctx, Batcher* q, Batch* b) {
 }
 int32_t dbsp_batcher_new(dbsp_ctx* ctx, const dbsp_schema* s, dbsp_batcher** out) {
   NOT_NULL(ctx, "ctx");
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_schema(s, WHAT));
+  REFUSE(dv::check_new(WHAT, out, s));
   Batcher* q = new Batcher();
   q->s = *s;
   *out = (dbsp_batcher*)q;
@@ -762,10 +687,8 @@ int32_t dbsp_batcher_new(dbsp_ctx* ctx, const dbsp_schema* s, dbsp_batcher** out
 }
 int32_t dbsp_batcher_push(dbsp_ctx* ctx, dbsp_batcher* bq, const uint64_t* const* cols, const int64_t* w, uint64_t n,
                           int32_t on_device) { ENTER(ctx);
-  NOT_NULL(bq, "batcher");
   Batcher* q = (Batcher*)bq;
-  REFUSE(valid_cols(WHAT, cols, q->s.n_key_lanes + q->s.n_val_lanes, n));
-  ROWS32(n);
+  REFUSE(dv::check_push(WHAT, q ? &q->s : nullptr, cols, w, n, false));
   if (n == 0) return DBSP_OK;
   dbsp_batch* b = nullptr;
   TRY(dbsp_batch_from_tuples(ctx, &q->s, cols, w, n, on_device, &b));
@@ -773,12 +696,9 @@ int32_t dbsp_batcher_push(dbsp_ctx* ctx, dbsp_batcher* bq, const uint64_t* const
 }
 int32_t dbsp_batcher_push_consolidated(dbsp_ctx* ctx, dbsp_batcher* bq, const uint64_t* const* cols, const int64_t* w,
                                        uint64_t n, int32_t on_device) { ENTER(ctx);
-  NOT_NULL(bq, "batcher");
   Batcher* q = (Batcher*)bq;
-  REFUSE(valid_cols(WHAT, cols, q->s.n_key_lanes + q->s.n_val_lanes, n));
-  ROWS32(n);
+  REFUSE(dv::check_push(WHAT, q ? &q->s : nullptr, cols, w, n, true));
   if (n == 0) return DBSP_OK;
-  CHECK_ARG(w != nullptr, "batcher_push_consolidated: weights is NULL (consolidated rows carry their weights)");
   dbsp_batch* b = nullptr;
   TRY(dbsp_batch_from_sorted(ctx, &q->s, cols, w, n, on_device, &b));
   return batcher_enqueue(ctx, q, B(b));
@@ -820,17 +740,13 @@ int32_t dbsp_batcher_seal(dbsp_ctx* ctx, dbsp_batcher* bq, dbsp_batch** out) { E
 }
 
 int32_t dbsp_batch_empty(dbsp_ctx* ctx, const dbsp_schema* s, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_schema(s, WHAT));
+  REFUSE(dv::check_new(WHAT, out, s));
   *out = H(batch_new_empty(ctx, *s));
   return DBSP_OK;
 }
 
 int32_t dbsp_batch_merge(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(a, "a");
-  NOT_NULL(b, "b");
-  CHECK_ARG(dv::same_schema(B(a)->s, B(b)->s), std::string(WHAT) + ": a and b differ in schema");
+  REFUSE(dv::check_merge(WHAT, out, S(a), S(b)));
   Batch* o = nullptr;
   TRY(merge_batches(ctx, B(a), B(b), &o));
   *out = H(o);
@@ -839,10 +755,7 @@ int32_t dbsp_batch_merge(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b
 
 int32_t dbsp_batch_merge_bounded(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b, const uint64_t* vb,
                                  dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(a, "a");
-  NOT_NULL(b, "b");
-  CHECK_ARG(dv::same_schema(B(a)->s, B(b)->s), std::string(WHAT) + ": a and b differ in schema");
+  REFUSE(dv::check_merge(WHAT, out, S(a), S(b)));
   Batch* o = nullptr;
   TRY(merge_bounded(ctx, B(a), B(b), vb, &o));
   *out = H(o);
@@ -850,9 +763,7 @@ int32_t dbsp_batch_merge_bounded(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_
 }
 
 int32_t dbsp_batch_truncate_keys_below(dbsp_ctx* ctx, const dbsp_batch* b, const uint64_t* key, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
-  CHECK_ARG(key != nullptr || B(b)->s.n_key_lanes == 0, "batch_truncate_keys_below: key is NULL");
+  REFUSE(dv::check_truncate(out, S(b), key));
   u64 pos;
   TRY(batch_lower_bound(ctx, B(b), key, &pos));
   if (pos == 0) { batch_ref(B(b)); *out = (dbsp_batch*)b; return DBSP_OK; }
@@ -861,10 +772,7 @@ int32_t dbsp_batch_truncate_keys_below(dbsp_ctx* ctx, const dbsp_batch* b, const
 }
 
 int32_t dbsp_merger_new(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b, const uint64_t* vb, dbsp_merger** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(a, "a");
-  NOT_NULL(b, "b");
-  CHECK_ARG(dv::same_schema(B(a)->s, B(b)->s), std::string(WHAT) + ": a and b differ in schema");
+  REFUSE(dv::check_merge(WHAT, out, S(a), S(b)));
   Merger* m = new Merger();
   m->ctx = ctx;
   m->a = B(a);
@@ -914,10 +822,8 @@ int32_t dbsp_merger_free(dbsp_merger* mm) {
 }
 
 int32_t dbsp_merger_done(dbsp_ctx* ctx, dbsp_merger* mm, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(mm, "merger");
-  NOT_NULL(out, "out");
   Merger* m = (Merger*)mm;
-  CHECK_ARG(m->complete(), "merger_done: merger: the merge is not complete (merger_work left fuel <= 0)");
+  REFUSE(dv::check_merger_done(m, m && m->complete(), out));
   Batch* o = nullptr;
   TRY(batch_concat(ctx, m->a->s, m->chunks, &o));   // on failure the merger stays owned by the caller
   dbsp_merger_free(mm);
@@ -935,10 +841,8 @@ int32_t dbsp_batch_neg(dbsp_ctx* ctx, const dbsp_batch* a, dbsp_batch** out) { E
 }
 
 int32_t dbsp_batch_reindex(dbsp_ctx* ctx, const dbsp_batch* a, uint32_t nk, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(a, "batch");
+  REFUSE(dv::check_reindex(out, S(a), nk));
   const Batch* x = B(a);
-  CHECK_ARG(nk <= (uint32_t)x->nl(), "batch_reindex: n_key_lanes = " + std::to_string(nk) + ": the batch has " + std::to_string(x->nl()) + " lanes");
   Batch* v = new Batch();
   v->s = x->s;
   v->s.n_key_lanes = (uint8_t)nk;
@@ -1077,9 +981,7 @@ int32_t dbsp_batch_device_columns(const dbsp_batch* b, const uint64_t** cols, co
 }
 
 int32_t dbsp_batch_last_key(dbsp_ctx* ctx, const dbsp_batch* b, uint64_t* key, int32_t* valid) { ENTER(ctx);
-  NOT_NULL(b, "batch");
-  NOT_NULL(valid, "valid");
-  CHECK_ARG(key != nullptr || B(b)->s.n_key_lanes == 0, "batch_last_key: key is NULL");
+  REFUSE(dv::check_last_key(S(b), key, valid));
   const Batch* x = B(b);
   *valid = x->n > 0;
   if (!x->n) return DBSP_OK;
@@ -1105,8 +1007,7 @@ int32_t dbsp_batch_free(dbsp_batch* b) {
 }
 
 int32_t dbsp_spine_new(dbsp_ctx* ctx, const dbsp_schema* s, dbsp_spine** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_schema(s, WHAT));
+  REFUSE(dv::check_new(WHAT, out, s));
   dbsp_spine* sp = new dbsp_spine();
   sp->s = *s;
   sp->ctx = ctx;
@@ -1114,9 +1015,7 @@ int32_t dbsp_spine_new(dbsp_ctx* ctx, const dbsp_schema* s, dbsp_spine** out) { 
   return DBSP_OK;
 }
 int32_t dbsp_spine_insert(dbsp_ctx* ctx, dbsp_spine* s, const dbsp_batch* b) { ENTER(ctx);
-  NOT_NULL(s, "spine");
-  NOT_NULL(b, "batch");
-  CHECK_ARG(dv::same_schema(s->s, B(b)->s), "spine_insert: spine and batch differ in schema");
+  REFUSE(dv::check_spine_insert(S(s), S(b)));
   return spine_insert(ctx, s, B(b));
 }
 int32_t dbsp_spine_consolidate(dbsp_ctx* ctx, dbsp_spine* s, dbsp_batch** out) { ENTER(ctx);
@@ -1137,8 +1036,7 @@ int32_t dbsp_spine_consolidate(dbsp_ctx* ctx, dbsp_spine* s, dbsp_batch** out) {
   return DBSP_OK;
 }
 int32_t dbsp_spine_truncate_keys_below(dbsp_ctx* ctx, dbsp_spine* s, const uint64_t* key) { ENTER(ctx);
-  NOT_NULL(s, "spine");
-  CHECK_ARG(key != nullptr || s->s.n_key_lanes == 0, "spine_truncate_keys_below: key is NULL");
+  REFUSE(dv::check_truncate(WHAT, S(s), key, false));
   bool raise = !s->has_bound;
   if (!raise) {   // the bound only grows (spine_fueled.rs:223-233)
     for (int l = 0; l < s->s.n_key_lanes; l++) {
@@ -1164,8 +1062,7 @@ int32_t dbsp_spine_truncate_keys_below(dbsp_ctx* ctx, dbsp_spine* s, const uint6
 }
 int32_t dbsp_spine_truncate_values_below(dbsp_ctx* ctx, dbsp_spine* s, const uint64_t* val) {
   NOT_NULL(ctx, "ctx");
-  NOT_NULL(s, "spine");
-  CHECK_ARG(val != nullptr || s->s.n_val_lanes == 0, "spine_truncate_values_below: val is NULL");
+  REFUSE(dv::check_truncate(WHAT, S(s), val, true));
   int nk = s->s.n_key_lanes, nv = s->s.n_val_lanes;
   bool raise = !s->has_vbound;
   if (!raise) {   // the bound only grows (spine_fueled.rs:644-652)
@@ -1337,73 +1234,36 @@ int32_t dbsp_spine_load(dbsp_ctx* ctx, const char* path, dbsp_spine** out) { ENT
   *out = H(o__);              \
   return DBSP_OK;
 
-// the two sides of a join: equal key lanes; proj reads the key, the left values and the right values
-static std::string valid_join(const char* what, const dbsp_schema& left, const dbsp_schema& right, const dbsp_proj* p) {
-  if (!dv::same_key_lanes(left, right)) return std::string(what) + ": the two inputs differ in key lanes (count or type)";
-  return dv::valid_proj(p, left.n_key_lanes, left.n_val_lanes, right.n_val_lanes, what);
-}
-static std::string valid_join_fn(const char* what, const dbsp_schema& left, const dbsp_schema& right, const dbsp_rowfn* f) {
-  if (!dv::same_key_lanes(left, right)) return std::string(what) + ": the two inputs differ in key lanes (count or type)";
-  return dv::valid_rowfn(f, left.n_key_lanes, left.n_val_lanes, right.n_val_lanes, what);
-}
-
 int32_t dbsp_join_delta_trace(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* t, const dbsp_proj* p, int32_t dl,
                               dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(d, "delta");
-  NOT_NULL(t, "trace");
-  REFUSE(dl ? valid_join(WHAT, B(d)->s, t->s, p) : valid_join(WHAT, t->s, B(d)->s, p));
+  REFUSE(dv::check_join(WHAT, out, S(d), S(t), dl, p));
   OUT1(op_join_delta_trace(ctx, B(d), t, p, dl, &o__)) }
 int32_t dbsp_join_batches(dbsp_ctx* ctx, const dbsp_batch* l, const dbsp_batch* r, const dbsp_proj* p, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(l, "left");
-  NOT_NULL(r, "right");
-  REFUSE(valid_join(WHAT, B(l)->s, B(r)->s, p));
+  REFUSE(dv::check_join(WHAT, out, S(l), S(r), p));
   OUT1(op_join_batches(ctx, B(l), B(r), p, &o__)) }
 int32_t dbsp_join_delta_trace_fn(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* t, const dbsp_rowfn* f, int32_t dl,
                                  dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(d, "delta");
-  NOT_NULL(t, "trace");
-  REFUSE(dl ? valid_join_fn(WHAT, B(d)->s, t->s, f) : valid_join_fn(WHAT, t->s, B(d)->s, f));
+  REFUSE(dv::check_join(WHAT, out, S(d), S(t), dl, f));
   OUT1(op_join_delta_trace(ctx, B(d), t, f, dl, &o__)) }
 int32_t dbsp_join_batches_fn(dbsp_ctx* ctx, const dbsp_batch* l, const dbsp_batch* r, const dbsp_rowfn* f, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(l, "left");
-  NOT_NULL(r, "right");
-  REFUSE(valid_join_fn(WHAT, B(l)->s, B(r)->s, f));
+  REFUSE(dv::check_join(WHAT, out, S(l), S(r), f));
   OUT1(op_join_batches(ctx, B(l), B(r), f, &o__)) }
 int32_t dbsp_semijoin(dbsp_ctx* ctx, const dbsp_batch* pairs, const dbsp_batch* keys, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(pairs, "pairs");
-  NOT_NULL(keys, "keys");
-  CHECK_ARG(dv::same_key_lanes(B(pairs)->s, B(keys)->s), "semijoin: pairs and keys differ in key lanes (count or type)");
-  CHECK_ARG(B(keys)->s.n_val_lanes == 0, "semijoin: keys must be a batch without value lanes");
+  REFUSE(dv::check_semijoin(out, S(pairs), S(keys)));
   OUT1(op_semijoin(ctx, B(pairs), B(keys), &o__)) }
 int32_t dbsp_aggregate_delta(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* in_tr, const dbsp_spine* out_tr,
                              int32_t kind, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(d, "delta");
-  NOT_NULL(in_tr, "in_trace");
-  NOT_NULL(out_tr, "out_trace");
-  REFUSE(dv::valid_aggregate(B(d)->s, in_tr->s, out_tr->s, kind));
+  REFUSE(dv::valid_aggregate(out, S(d), S(in_tr), S(out_tr), kind));
   OUT1(op_aggregate_delta(ctx, B(d), in_tr, out_tr, kind, &o__)) }
 int32_t dbsp_aggregate_fold(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* in_tr, const dbsp_spine* out_tr,
                             const dbsp_fold* fold, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(d, "delta");
-  NOT_NULL(in_tr, "in_trace");
-  NOT_NULL(out_tr, "out_trace");
-  REFUSE(dv::valid_fold(B(d)->s, in_tr->s, out_tr->s, fold));
+  REFUSE(dv::valid_fold(out, S(d), S(in_tr), S(out_tr), fold));
   OUT1(op_aggregate_fold(ctx, B(d), in_tr, out_tr, fold, &o__)) }
 int32_t dbsp_upsert_commands(dbsp_ctx* ctx, const dbsp_schema* table, const uint64_t* const* cols,
                              const uint8_t* insert, uint64_t n, uint64_t seq0, int32_t on_device,
                              dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_upsert(table, n, seq0));
+  REFUSE(dv::valid_upsert(out, table, cols, n, seq0));
   const int L = table->n_key_lanes + table->n_val_lanes;
-  REFUSE(valid_cols(WHAT, cols, L, n));
-  ROWS32(n);
   BufP hold, ihold;
   Cols dc;
   const i64* dw;
@@ -1417,42 +1277,20 @@ int32_t dbsp_upsert_commands(dbsp_ctx* ctx, const dbsp_schema* table, const uint
   }
   OUT1(op_upsert_commands(ctx, *table, dc, dins, n, seq0, &o__)) }
 int32_t dbsp_upsert_delta(dbsp_ctx* ctx, const dbsp_batch* cmds, const dbsp_spine* table, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(cmds, "cmds");
-  NOT_NULL(table, "table");
-  REFUSE(dv::valid_upsert(B(cmds)->s, table->s));
+  REFUSE(dv::valid_upsert(out, S(cmds), S(table)));
   OUT1(op_upsert_delta(ctx, B(cmds), table, &o__)) }
 int32_t dbsp_weigh(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_expr* f, int32_t mode, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
-  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || mode == DBSP_WEIGH_AVG, "weigh: mode = " + std::to_string(mode) + " is not a weigh mode");
-  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || B(b)->s.n_key_lanes < MAXL, "weigh: WEIGH_AVG adds a key lane and the batch already has 8");
-  CHECK_ARG(mode == DBSP_WEIGH_AVG || B(b)->s.n_key_lanes >= 1, "weigh: WEIGH_LINEAR of a batch without key lanes has no output lanes");
-  REFUSE(dv::valid_expr(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, "weigh: f"));
+  REFUSE(dv::check_weigh(out, S(b), f, mode));
   OUT1(op_weigh(ctx, B(b), f, mode, &o__)) }
 int32_t dbsp_weigh_fn(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_rowfn* f, int32_t mode, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
-  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || mode == DBSP_WEIGH_AVG, "weigh_fn: mode = " + std::to_string(mode) + " is not a weigh mode");
-  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || B(b)->s.n_key_lanes < MAXL, "weigh_fn: WEIGH_AVG adds a key lane and the batch already has 8");
-  CHECK_ARG(mode == DBSP_WEIGH_AVG || B(b)->s.n_key_lanes >= 1, "weigh_fn: WEIGH_LINEAR of a batch without key lanes has no output lanes");
-  REFUSE(dv::valid_rowfn(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT));
-  CHECK_ARG(f->out_schema.n_key_lanes + f->out_schema.n_val_lanes == 1, "weigh_fn: fn.out_schema must have one lane (the factor)");
+  REFUSE(dv::check_weigh(out, S(b), f, mode));
   OUT1(op_weigh(ctx, B(b), f, mode, &o__)) }
 int32_t dbsp_distinct_delta(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* i, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(d, "delta");
-  NOT_NULL(i, "delayed_integral");
-  CHECK_ARG(dv::same_schema(B(d)->s, i->s), "distinct_delta: delta and delayed_integral differ in schema");
+  REFUSE(dv::check_distinct_delta(out, S(d), S(i)));
   OUT1(op_distinct_delta(ctx, B(d), i, &o__)) }
 int32_t dbsp_antijoin_delta(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* t, const dbsp_batch* kd,
                             const dbsp_spine* kt, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(d, "delta");
-  NOT_NULL(t, "trace");
-  NOT_NULL(kd, "key_delta");
-  NOT_NULL(kt, "key_trace");
-  REFUSE(dv::valid_antijoin(B(d)->s, t->s, B(kd)->s, kt->s));
+  REFUSE(dv::valid_antijoin(out, S(d), S(t), S(kd), S(kt)));
   OUT1(op_antijoin_delta(ctx, B(d), t, B(kd), kt, &o__)) }
 int32_t dbsp_stream_distinct(dbsp_ctx* ctx, const dbsp_batch* b, dbsp_batch** out) { ENTER(ctx);
   NOT_NULL(out, "out");
@@ -1460,36 +1298,21 @@ int32_t dbsp_stream_distinct(dbsp_ctx* ctx, const dbsp_batch* b, dbsp_batch** ou
   OUT1(op_stream_distinct(ctx, B(b), &o__)) }
 int32_t dbsp_window_delta(dbsp_ctx* ctx, const dbsp_spine* t, const dbsp_batch* d, int32_t has_prev, const uint64_t* s0,
                           const uint64_t* e0, const uint64_t* s1, const uint64_t* e1, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(t, "trace");
-  NOT_NULL(d, "delta");
-  CHECK_ARG(dv::same_schema(t->s, B(d)->s), "window_delta: trace and delta differ in schema");
-  CHECK_ARG(s1 && e1, "window_delta: start1 / end1 is NULL");
-  CHECK_ARG(!has_prev || (s0 && e0), "window_delta: start0 / end0 is NULL although has_prev is set");
+  REFUSE(dv::check_window_delta(out, S(t), S(d), has_prev, s0, e0, s1, e1));
   if (!has_prev) { s0 = s1; e0 = e1; }   // never read by the operator's logic; keeps the copies below defined
   OUT1(op_window_delta(ctx, t, B(d), has_prev, s0, e0, s1, e1, &o__)) }
 int32_t dbsp_map_index(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_proj* p, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
-  REFUSE(dv::valid_proj(p, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT));
+  REFUSE(dv::check_map_index(WHAT, out, S(b), p));
   OUT1(op_map_index(ctx, B(b), p, &o__)) }
 int32_t dbsp_map_index_fn(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_rowfn* f, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
-  REFUSE(dv::valid_rowfn(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT));
+  REFUSE(dv::check_map_index(WHAT, out, S(b), f));
   OUT1(op_map_index(ctx, B(b), f, &o__)) }
 int32_t dbsp_map_index_fanout(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_rowfn* f, uint32_t n_out, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
-  REFUSE(dv::valid_fanout(n_out, WHAT));
-  REFUSE(dv::valid_rowfn(f, B(b)->s.n_key_lanes, B(b)->s.n_val_lanes, B(b)->s.n_val_lanes, WHAT, dv::SRC_BIT_FANOUT));
-  FANOUT_ROWS(B(b)->n, n_out);
+  REFUSE(dv::check_map_index(WHAT, out, S(b), b ? B(b)->n : 0, f, n_out));
   const RowFnFanout fo = fanout_of(*f, n_out);
   OUT1(op_map_index(ctx, B(b), &fo, &o__)) }
 int32_t dbsp_shard_partition(dbsp_ctx* ctx, const dbsp_batch* b, uint32_t P, dbsp_batch** outs) { ENTER(ctx);
-  NOT_NULL(b, "batch");
-  NOT_NULL(outs, "outs");
-  CHECK_ARG(P >= 1 && P <= 64, "shard_partition: n_shards = " + std::to_string(P) + ": 1..64 shards");
+  REFUSE(dv::check_shard_partition(S(b), outs, P));
   std::vector<Batch*> o(P, nullptr);
   const int32_t rc = op_shard_partition(ctx, B(b), P, o.data());
   if (rc != DBSP_OK) {
@@ -1501,13 +1324,11 @@ int32_t dbsp_shard_partition(dbsp_ctx* ctx, const dbsp_batch* b, uint32_t P, dbs
 }
 
 int32_t dbsp_comm_create(dbsp_ctx* ctx, int32_t rank, int32_t world, uint64_t slot_bytes, uint8_t* blob_out) { ENTER(ctx);
-  CHECK_ARG(blob_out != nullptr, "comm_create: blob_out is NULL");
-  CHECK_ARG(world >= 1 && world <= DBSP_COMM_MAX_RANKS, "comm_create: world = " + std::to_string(world) + ": 1..32 ranks");
-  CHECK_ARG(rank >= 0 && rank < world, "comm_create: rank = " + std::to_string(rank) + " is not below world = " + std::to_string(world));
+  REFUSE(dv::check_comm_create(rank, world, blob_out));
   return comm_create(ctx, rank, world, slot_bytes, blob_out);
 }
 int32_t dbsp_comm_connect(dbsp_ctx* ctx, const uint8_t* blobs) { ENTER(ctx);
-  CHECK_ARG(blobs != nullptr, "comm_connect: blobs is NULL");
+  NOT_NULL(blobs, "blobs");
   return comm_connect(ctx, blobs);
 }
 int32_t dbsp_comm_destroy(dbsp_ctx* ctx) { ENTER(ctx);
@@ -1547,11 +1368,9 @@ int32_t dbsp_shard2(dbsp_ctx* ctx, const dbsp_batch* a, const dbsp_batch* b, dbs
   return DBSP_OK;
 }
 int32_t dbsp_gather(dbsp_ctx* ctx, const dbsp_batch* b, int32_t root, dbsp_batch** out) { ENTER(ctx);
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
   int r, w;
   comm_info(ctx, &r, &w, nullptr);
-  CHECK_ARG(root >= 0 && root < w, "gather: root = " + std::to_string(root) + " is not a rank of a group of " + std::to_string(w));
+  REFUSE(dv::check_gather(out, S(b), root, w));
   const Batch* in[1] = {B(b)};
   Batch* o[1] = {nullptr};
   TRY(comm_exchange(ctx, in, 1, root, o));

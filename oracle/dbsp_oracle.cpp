@@ -723,43 +723,24 @@ static thread_local std::string g_err;
 
 static orc_batch* wrap(BatchP p) { return new orc_batch{p}; }
 
-// The error contract of include/dbsp_b200.h, with the CUDA library's rules and texts (validate.h): every argument is
-// checked before the call reads or builds anything.  WHAT is the call's name without the prefix.
+// The error contract of include/dbsp_b200.h: every argument is checked, by the call's check in validate.h (the CUDA
+// library's), before the call reads or builds anything.  WHAT is the call's name without the prefix.
 namespace dv = dbsp_validate;
-#define CHECK_ARG(c, msg)                                  \
-  do {                                                     \
-    if (!(c)) { g_err = (msg); return DBSP_ERR_INVALID; } \
-  } while (0)
 #define WHAT (__func__ + 4)
-#define NOT_NULL(p, name) CHECK_ARG((p) != nullptr, std::string(WHAT) + ": " name " is NULL")
-#define REFUSE(text)                                               \
-  do {                                                             \
-    const std::string m__ = (text);                                \
-    if (!m__.empty()) { g_err = m__; return DBSP_ERR_INVALID; }   \
+#define REFUSE(check)                                       \
+  do {                                                      \
+    const dv::Refusal r__ = (check);                        \
+    if (r__) { g_err = r__.text; return r__.status; }       \
   } while (0)
-#define ROWS32(n)                                                                                \
-  do {                                                                                           \
-    if ((u64)(n) >= 0xffffffffull) {                                                             \
-      g_err = std::string(WHAT) + ": n = " + std::to_string(n) + ": 2^32-1 or more rows in one batch; split the batch"; \
-      return DBSP_ERR_UNSUPPORTED;                                                               \
-    }                                                                                            \
-  } while (0)
-static std::string valid_cols(const char* what, const u64* const* cols, int ncols, u64 n, unsigned mask = ~0u) {
-  if (!cols) return std::string(what) + ": cols is NULL";
-  for (int l = 0; n && l < ncols; l++)
-    if (((mask >> l) & 1) && !cols[l]) return std::string(what) + ": cols[" + std::to_string(l) + "] is NULL";
-  return "";
-}
-static std::string valid_join(const char* what, const dbsp_schema& left, const dbsp_schema& right, const dbsp_proj* p) {
-  if (!dv::same_key_lanes(left, right)) return std::string(what) + ": the two inputs differ in key lanes (count or type)";
-  return dv::valid_proj(p, left.n_key_lanes, left.n_val_lanes, right.n_val_lanes, what);
-}
+#define NOT_NULL(p, name) REFUSE(dv::not_null(p, WHAT, name))
+// a handle's schema as the checks of validate.h take it: NULL for a NULL handle
+static const dbsp_schema* S(const orc_batch* b) { return b ? &b->p->s : nullptr; }
+static const dbsp_schema* S(const orc_spine* s) { return s ? &s->s.s : nullptr; }
 
 extern "C" {
 
 int32_t orc_ctx_create(int32_t device, orc_ctx** out) {
-  NOT_NULL(out, "out");
-  CHECK_ARG(device >= 0, "ctx_create: device is negative");
+  REFUSE(dv::check_ctx_create(out, device));
   *out = new orc_ctx{0};
   return DBSP_OK;
 }
@@ -768,28 +749,24 @@ int32_t orc_ctx_sync(orc_ctx* c) { NOT_NULL(c, "ctx"); return DBSP_OK; }
 const char* orc_last_error(void) { return g_err.c_str(); }
 int32_t orc_ctx_stats(orc_ctx* ctx, u64* a, u64* b, u64* c, int32_t) { NOT_NULL(ctx, "ctx"); if (a) *a = 0; if (b) *b = 0; if (c) *c = 0; return DBSP_OK; }
 void* orc_ctx_stream(orc_ctx*) { return nullptr; }
-int32_t orc_ctx_profile(orc_ctx* c, int32_t) { NOT_NULL(c, "ctx"); return DBSP_OK; }
+int32_t orc_ctx_profile(orc_ctx* c, int32_t enable) {
+  NOT_NULL(c, "ctx");
+  REFUSE(dv::check_ctx_profile(enable));
+  return DBSP_OK;
+}
 int32_t orc_ctx_profile_read(orc_ctx*, int32_t, char*, u64*, double*, u64*) { return DBSP_ERR_INVALID; }
 
 int32_t orc_batch_from_tuples(orc_ctx* c, const dbsp_schema* s, const u64* const* cols, const i64* w, u64 n,
                               int32_t, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_schema(s, WHAT));
-  REFUSE(valid_cols(WHAT, cols, s->n_key_lanes + s->n_val_lanes, n));
-  ROWS32(n);
+  REFUSE(dv::check_tuples(WHAT, out, s, cols, w, n, false));
   *out = wrap(from_tuples(*s, cols, w, n));
   return DBSP_OK;
 }
 
 // FlatMap::eval + from_tuples (operator/filter_map.rs:700-724).
-static int32_t table_to_batch(const char* what, const u64* const* cols, uint32_t ncols, unsigned col_mask, const i64* w, u64 n,
-                              const dbsp_proj* proj, orc_batch** out) {
-  REFUSE(dv::valid_proj(proj, (int)ncols, (int)ncols, (int)ncols, what));
+static void table_to_batch(const u64* const* cols, uint32_t ncols, const i64* w, u64 n, const dbsp_proj* proj, orc_batch** out) {
   const unsigned used = dv::proj_table_mask(*proj);
-  CHECK_ARG((used & ~col_mask) == 0, std::string(what) + ": proj reads column " + std::to_string(__builtin_ctz((used & ~col_mask) | 0x100u)) +
-                                         ", which col_mask left out of the upload");
-  REFUSE(valid_cols(what, cols, (int)ncols, n, used));
   Tuples t(proj->out_schema);
   u64 lv[MAXL] = {0}, row[MAXL];
   for (u64 i = 0; i < n; i++) {
@@ -798,57 +775,49 @@ static int32_t table_to_batch(const char* what, const u64* const* cols, uint32_t
     if (project(*proj, e, row)) t.push(row, w ? w[i] : 1);
   }
   *out = wrap(t.build());
-  return DBSP_OK;
 }
 int32_t orc_batch_from_table(orc_ctx* c, const u64* const* cols, uint32_t ncols, const i64* w, u64 n, int32_t,
                              const dbsp_proj* proj, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  CHECK_ARG(ncols >= 1 && ncols <= MAXL, "batch_from_table: n_cols = " + std::to_string(ncols) + ": a table has 1..8 columns");
-  ROWS32(n);
-  return table_to_batch(WHAT, cols, ncols, ~0u, w, n, proj, out);
+  REFUSE(dv::check_table(WHAT, out, cols, ncols, n, proj));
+  table_to_batch(cols, ncols, w, n, proj, out);
+  return DBSP_OK;
 }
 
 // pipelined ingest: on the CPU there is nothing to overlap, keep the pointers
-struct orc_upload { const u64* const* cols; uint32_t n_cols; uint32_t col_mask; const i64* w; u64 n; std::vector<const u64*> own; };
+struct orc_upload { const orc_ctx* ctx; const u64* const* cols; uint32_t n_cols; uint32_t col_mask; const i64* w; u64 n; std::vector<const u64*> own; };
+static dv::Upload upload_of(const orc_upload* u, const orc_ctx* c) {
+  if (!u) return dv::Upload{false, false, 0, 0, 0};
+  return dv::Upload{true, u->ctx == c, (int)u->n_cols, u->col_mask, u->n};
+}
 int32_t orc_upload_begin(orc_ctx* c, const u64* const* cols, uint32_t n_cols, uint32_t col_mask, const i64* w, u64 n, orc_upload** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  CHECK_ARG(n_cols >= 1 && n_cols <= MAXL, "upload_begin: n_cols = " + std::to_string(n_cols) + ": a table has 1..8 columns");
-  REFUSE(valid_cols(WHAT, cols, (int)n_cols, n, col_mask));
-  ROWS32(n);
+  REFUSE(dv::check_upload_begin(out, cols, n_cols, col_mask, n));
   orc_upload* u = new orc_upload();
   u->own.assign(cols, cols + n_cols);
-  u->cols = u->own.data(); u->n_cols = n_cols; u->col_mask = col_mask; u->w = w; u->n = n;
+  u->ctx = c; u->cols = u->own.data(); u->n_cols = n_cols; u->col_mask = col_mask; u->w = w; u->n = n;
   *out = u;
   return DBSP_OK;
 }
 int32_t orc_batch_from_upload(orc_ctx* c, orc_upload* u, const dbsp_proj* proj, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(u, "upload");
-  return table_to_batch(WHAT, u->cols, u->n_cols, u->col_mask, u->w, u->n, proj, out);
+  REFUSE(dv::check_upload(WHAT, out, upload_of(u, c), proj));
+  table_to_batch(u->cols, u->n_cols, u->w, u->n, proj, out);
+  return DBSP_OK;
 }
 int32_t orc_upload_free(orc_upload* u) { delete u; return DBSP_OK; }
-uint32_t orc_proj_table_mask(const dbsp_proj* proj) {
-  if (!dv::valid_proj(proj, MAXL, MAXL, MAXL, "proj_table_mask").empty()) return 0;
-  return dv::proj_table_mask(*proj);
-}
+uint32_t orc_proj_table_mask(const dbsp_proj* proj) { return dv::checked_table_mask(proj, WHAT); }
 
 int32_t orc_batch_empty(orc_ctx* c, const dbsp_schema* s, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_schema(s, WHAT));
+  REFUSE(dv::check_new(WHAT, out, s));
   *out = wrap(std::make_shared<Batch>(*s));
   return DBSP_OK;
 }
 
 int32_t orc_batch_merge(orc_ctx* c, const orc_batch* a, const orc_batch* b, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(a, "a");
-  NOT_NULL(b, "b");
-  CHECK_ARG(dv::same_schema(a->p->s, b->p->s), std::string(WHAT) + ": a and b differ in schema");
+  REFUSE(dv::check_merge(WHAT, out, S(a), S(b)));
   *out = wrap(merge(a->p, b->p));
   return DBSP_OK;
 }
@@ -870,16 +839,13 @@ static void batcher_enqueue(orc_batcher* q, BatchP b) {
 }
 int32_t orc_batcher_new(orc_ctx* c, const dbsp_schema* s, orc_batcher** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_schema(s, WHAT));
+  REFUSE(dv::check_new(WHAT, out, s));
   *out = new orc_batcher{*s, {}};
   return DBSP_OK;
 }
 int32_t orc_batcher_push(orc_ctx* c, orc_batcher* q, const u64* const* cols, const i64* w, u64 n, int32_t) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(q, "batcher");
-  REFUSE(valid_cols(WHAT, cols, q->s.n_key_lanes + q->s.n_val_lanes, n));
-  ROWS32(n);
+  REFUSE(dv::check_push(WHAT, q ? &q->s : nullptr, cols, w, n, false));
   if (n) batcher_enqueue(q, from_tuples(q->s, cols, w, n));
   return DBSP_OK;
 }
@@ -887,11 +853,8 @@ int32_t orc_batch_from_sorted(orc_ctx* c, const dbsp_schema* s, const u64* const
                               orc_batch** out);
 int32_t orc_batcher_push_consolidated(orc_ctx* c, orc_batcher* q, const u64* const* cols, const i64* w, u64 n, int32_t od) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(q, "batcher");
-  REFUSE(valid_cols(WHAT, cols, q->s.n_key_lanes + q->s.n_val_lanes, n));
-  ROWS32(n);
+  REFUSE(dv::check_push(WHAT, q ? &q->s : nullptr, cols, w, n, true));
   if (!n) return DBSP_OK;
-  CHECK_ARG(w != nullptr, "batcher_push_consolidated: weights is NULL (consolidated rows carry their weights)");
   orc_batch* b = nullptr;
   int32_t rc = orc_batch_from_sorted(c, &q->s, cols, w, n, od, &b);
   if (rc) return rc;
@@ -921,20 +884,14 @@ int32_t orc_batcher_seal(orc_ctx* c, orc_batcher* q, orc_batch** out) {
 // bound (zset_batch.rs:307-318).
 int32_t orc_batch_merge_bounded(orc_ctx* c, const orc_batch* a, const orc_batch* b, const u64* vb, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(a, "a");
-  NOT_NULL(b, "b");
-  CHECK_ARG(dv::same_schema(a->p->s, b->p->s), std::string(WHAT) + ": a and b differ in schema");
+  REFUSE(dv::check_merge(WHAT, out, S(a), S(b)));
   *out = wrap(merge(a->p, b->p, a->p->indexed() ? vb : nullptr));
   return DBSP_OK;
 }
 struct orc_merger { Merger m; bool has_vb; u64 vb[MAXL]; };
 int32_t orc_merger_new(orc_ctx* c, const orc_batch* a, const orc_batch* b, const u64* vb, orc_merger** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(a, "a");
-  NOT_NULL(b, "b");
-  CHECK_ARG(dv::same_schema(a->p->s, b->p->s), std::string(WHAT) + ": a and b differ in schema");
+  REFUSE(dv::check_merge(WHAT, out, S(a), S(b)));
   orc_merger* m = new orc_merger{Merger(a->p, b->p), vb != nullptr && a->p->indexed(), {0}};
   if (m->has_vb) for (int l = 0; l < a->p->s.n_val_lanes; l++) m->vb[l] = vb[l];
   *out = m;
@@ -952,9 +909,7 @@ int32_t orc_merger_work(orc_ctx* c, orc_merger* m, i64* fuel) {
 }
 int32_t orc_merger_done(orc_ctx* c, orc_merger* m, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(m, "merger");
-  NOT_NULL(out, "out");
-  CHECK_ARG(m->m.complete(), "merger_done: merger: the merge is not complete (merger_work left fuel <= 0)");
+  REFUSE(dv::check_merger_done(m, m && m->m.complete(), out));
   *out = wrap(m->m.out);
   delete m;
   return DBSP_OK;
@@ -963,9 +918,7 @@ int32_t orc_merger_free(orc_merger* m) { delete m; return DBSP_OK; }
 // BatchReader::truncate_keys_below (trace/mod.rs:227-233).
 int32_t orc_batch_truncate_keys_below(orc_ctx* c, const orc_batch* b, const u64* key, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
-  CHECK_ARG(key != nullptr || b->p->s.n_key_lanes == 0, "batch_truncate_keys_below: key is NULL");
+  REFUSE(dv::check_truncate(out, S(b), key));
   BatchP t = truncate_keys_below(*b->p, key);
   *out = wrap(t ? t : b->p);
   return DBSP_OK;
@@ -999,11 +952,9 @@ static void flat_rows(const Batch& b, Tuples& t) {
 // index() (operator/index.rs:128-157) and its inverse: re-split the lanes.
 int32_t orc_batch_reindex(orc_ctx* c, const orc_batch* a, uint32_t nk, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(a, "batch");
+  REFUSE(dv::check_reindex(out, S(a), nk));
   dbsp_schema s = a->p->s;
   int nl = s.n_key_lanes + s.n_val_lanes;
-  CHECK_ARG(nk <= (uint32_t)nl, "batch_reindex: n_key_lanes = " + std::to_string(nk) + ": the batch has " + std::to_string(nl) + " lanes");
   s.n_key_lanes = nk; s.n_val_lanes = nl - nk;
   Tuples t(s);
   flat_rows(*a->p, t);
@@ -1045,9 +996,7 @@ int32_t orc_ctx_sync_stats(orc_ctx* c, u64* n, double* us, int32_t) { NOT_NULL(c
 // fast_forward_keys + get_key (operator/time_series/watermark.rs:38-45).
 int32_t orc_batch_last_key(orc_ctx* c, const orc_batch* b, u64* key, int32_t* valid) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(b, "batch");
-  NOT_NULL(valid, "valid");
-  CHECK_ARG(key != nullptr || b->p->s.n_key_lanes == 0, "batch_last_key: key is NULL");
+  REFUSE(dv::check_last_key(S(b), key, valid));
   const Batch& B = *b->p;
   *valid = B.K.n > 0;
   if (B.K.n) B.K.get(B.K.n - 1, key);
@@ -1061,11 +1010,7 @@ int32_t orc_batch_free(orc_batch* b) { delete b; return DBSP_OK; }
 int32_t orc_batch_from_sorted(orc_ctx* c, const dbsp_schema* s, const u64* const* cols, const i64* w, u64 n,
                               int32_t, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_schema(s, WHAT));
-  REFUSE(valid_cols(WHAT, cols, s->n_key_lanes + s->n_val_lanes, n));
-  CHECK_ARG(n == 0 || w != nullptr, "batch_from_sorted: weights is NULL (consolidated rows carry their weights)");
-  ROWS32(n);
+  REFUSE(dv::check_tuples(WHAT, out, s, cols, w, n, true));
   Builder bld(*s);
   const int nk = s->n_key_lanes, nv = s->n_val_lanes;
   u64 key[MAXL], val[MAXL];
@@ -1080,16 +1025,13 @@ int32_t orc_batch_from_sorted(orc_ctx* c, const dbsp_schema* s, const u64* const
 
 int32_t orc_spine_new(orc_ctx* c, const dbsp_schema* s, orc_spine** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_schema(s, WHAT));
+  REFUSE(dv::check_new(WHAT, out, s));
   *out = new orc_spine(*s);
   return DBSP_OK;
 }
 int32_t orc_spine_insert(orc_ctx* c, orc_spine* s, const orc_batch* b) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(s, "spine");
-  NOT_NULL(b, "batch");
-  CHECK_ARG(dv::same_schema(s->s.s, b->p->s), "spine_insert: spine and batch differ in schema");
+  REFUSE(dv::check_spine_insert(S(s), S(b)));
   s->s.insert(b->p);
   return DBSP_OK;
 }
@@ -1102,15 +1044,13 @@ int32_t orc_spine_consolidate(orc_ctx* c, orc_spine* s, orc_batch** out) {
 }
 int32_t orc_spine_truncate_keys_below(orc_ctx* c, orc_spine* s, const u64* key) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(s, "spine");
-  CHECK_ARG(key != nullptr || s->s.s.n_key_lanes == 0, "spine_truncate_keys_below: key is NULL");
+  REFUSE(dv::check_truncate(WHAT, S(s), key, false));
   s->s.truncate(key);
   return DBSP_OK;
 }
 int32_t orc_spine_truncate_values_below(orc_ctx* c, orc_spine* s, const u64* val) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(s, "spine");
-  CHECK_ARG(val != nullptr || s->s.s.n_val_lanes == 0, "spine_truncate_values_below: val is NULL");
+  REFUSE(dv::check_truncate(WHAT, S(s), val, true));
   s->s.truncate_values(val);
   return DBSP_OK;
 }
@@ -1136,10 +1076,7 @@ int32_t orc_spine_free(orc_spine* s) { delete s; return DBSP_OK; }
 int32_t orc_join_delta_trace(orc_ctx* c, const orc_batch* delta, const orc_spine* tr, const dbsp_proj* proj,
                              int32_t delta_is_left, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(delta, "delta");
-  NOT_NULL(tr, "trace");
-  REFUSE(delta_is_left ? valid_join(WHAT, delta->p->s, tr->s.s, proj) : valid_join(WHAT, tr->s.s, delta->p->s, proj));
+  REFUSE(dv::check_join(WHAT, out, S(delta), S(tr), delta_is_left, proj));
   Tuples t(proj->out_schema);
   for (auto& b : tr->s.batches) join_into(*delta->p, *b, *proj, !delta_is_left, t);
   *out = wrap(t.build());
@@ -1148,10 +1085,7 @@ int32_t orc_join_delta_trace(orc_ctx* c, const orc_batch* delta, const orc_spine
 
 int32_t orc_join_batches(orc_ctx* c, const orc_batch* l, const orc_batch* r, const dbsp_proj* proj, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(l, "left");
-  NOT_NULL(r, "right");
-  REFUSE(valid_join(WHAT, l->p->s, r->p->s, proj));
+  REFUSE(dv::check_join(WHAT, out, S(l), S(r), proj));
   Tuples t(proj->out_schema);
   join_into(*l->p, *r->p, *proj, false, t);
   *out = wrap(t.build());
@@ -1161,11 +1095,7 @@ int32_t orc_join_batches(orc_ctx* c, const orc_batch* l, const orc_batch* r, con
 // SemiJoinStream::eval (operator/semijoin.rs:100-142).
 int32_t orc_semijoin(orc_ctx* c, const orc_batch* pairs, const orc_batch* keys, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(pairs, "pairs");
-  NOT_NULL(keys, "keys");
-  CHECK_ARG(dv::same_key_lanes(pairs->p->s, keys->p->s), "semijoin: pairs and keys differ in key lanes (count or type)");
-  CHECK_ARG(keys->p->s.n_val_lanes == 0, "semijoin: keys must be a batch without value lanes");
+  REFUSE(dv::check_semijoin(out, S(pairs), S(keys)));
   const Batch& P = *pairs->p;
   const Batch& Kb = *keys->p;
   // Out: ZSet<Key = (Pairs::Key, Pairs::Val)> (semijoin.rs:47): an OrdZSet over all lanes
@@ -1203,11 +1133,7 @@ int32_t orc_semijoin(orc_ctx* c, const orc_batch* pairs, const orc_batch* keys, 
 int32_t orc_aggregate_delta(orc_ctx* c, const orc_batch* delta, const orc_spine* in_tr, const orc_spine* out_tr,
                             int32_t kind, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(delta, "delta");
-  NOT_NULL(in_tr, "in_trace");
-  NOT_NULL(out_tr, "out_trace");
-  REFUSE(dv::valid_aggregate(delta->p->s, in_tr->s.s, out_tr->s.s, kind));
+  REFUSE(dv::valid_aggregate(out, S(delta), S(in_tr), S(out_tr), kind));
   const Batch& D = *delta->p;
   const dbsp_schema& os = out_tr->s.s;
   int nk = os.n_key_lanes, nov = os.n_val_lanes;
@@ -1274,13 +1200,8 @@ int32_t orc_aggregate_delta(orc_ctx* c, const orc_batch* delta, const orc_spine*
 // weigh (operator/aggregate/mod.rs:297-323).
 int32_t orc_weigh(orc_ctx* c, const orc_batch* b, const dbsp_expr* f, int32_t mode, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
+  REFUSE(dv::check_weigh(out, S(b), f, mode));
   const Batch& B = *b->p;
-  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || mode == DBSP_WEIGH_AVG, "weigh: mode = " + std::to_string(mode) + " is not a weigh mode");
-  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || B.s.n_key_lanes < MAXL, "weigh: WEIGH_AVG adds a key lane and the batch already has 8");
-  CHECK_ARG(mode == DBSP_WEIGH_AVG || B.s.n_key_lanes >= 1, "weigh: WEIGH_LINEAR of a batch without key lanes has no output lanes");
-  REFUSE(dv::valid_expr(f, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, "weigh: f"));
   dbsp_schema s = B.s;
   s.n_val_lanes = 0;
   if (mode == DBSP_WEIGH_AVG) { s.lane_types[s.n_key_lanes] = DBSP_U64; s.n_key_lanes++; }
@@ -1311,10 +1232,7 @@ int32_t orc_weigh(orc_ctx* c, const orc_batch* b, const dbsp_expr* f, int32_t mo
 // DistinctIncrementalTotal::eval (operator/distinct.rs:196-254).
 int32_t orc_distinct_delta(orc_ctx* c, const orc_batch* delta, const orc_spine* integral, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(delta, "delta");
-  NOT_NULL(integral, "delayed_integral");
-  CHECK_ARG(dv::same_schema(delta->p->s, integral->s.s), "distinct_delta: delta and delayed_integral differ in schema");
+  REFUSE(dv::check_distinct_delta(out, S(delta), S(integral)));
   const Batch& D = *delta->p;
   Builder bld(D.s);
   std::vector<std::pair<KV, i64>> grp;
@@ -1363,12 +1281,7 @@ int32_t orc_stream_distinct(orc_ctx* c, const orc_batch* b, orc_batch** out) {
 int32_t orc_window_delta(orc_ctx* c, const orc_spine* tr, const orc_batch* delta, int32_t has_prev, const u64* s0,
                          const u64* e0, const u64* s1, const u64* e1, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(tr, "trace");
-  NOT_NULL(delta, "delta");
-  CHECK_ARG(dv::same_schema(tr->s.s, delta->p->s), "window_delta: trace and delta differ in schema");
-  CHECK_ARG(s1 && e1, "window_delta: start1 / end1 is NULL");
-  CHECK_ARG(!has_prev || (s0 && e0), "window_delta: start0 / end0 is NULL although has_prev is set");
+  REFUSE(dv::check_window_delta(out, S(tr), S(delta), has_prev, s0, e0, s1, e1));
   const dbsp_schema& s = delta->p->s;
   int nk = s.n_key_lanes;
   Tuples t(s);
@@ -1405,10 +1318,8 @@ int32_t orc_window_delta(orc_ctx* c, const orc_spine* tr, const orc_batch* delta
 // Map/FlatMap::eval + from_tuples (operator/filter_map.rs:563-577,700-724).
 int32_t orc_map_index(orc_ctx* c, const orc_batch* b, const dbsp_proj* proj, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
+  REFUSE(dv::check_map_index(WHAT, out, S(b), proj));
   const Batch& B = *b->p;
-  REFUSE(dv::valid_proj(proj, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, WHAT));
   Tuples t(proj->out_schema);
   u64 key[MAXL], val[MAXL] = {0}, row[MAXL];
   for (size_t k = 0; k < B.K.n; k++) {
@@ -1437,9 +1348,7 @@ static inline u64 mix64(u64 x) {
 // shard_batch (operator/communication/shard.rs:165-199).
 int32_t orc_shard_partition(orc_ctx* c, const orc_batch* b, uint32_t P, orc_batch** outs) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(b, "batch");
-  NOT_NULL(outs, "outs");
-  CHECK_ARG(P >= 1 && P <= 64, "shard_partition: n_shards = " + std::to_string(P) + ": 1..64 shards");
+  REFUSE(dv::check_shard_partition(S(b), outs, P));
   const Batch& B = *b->p;
   std::vector<Builder> blds;
   for (uint32_t p = 0; p < P; p++) blds.emplace_back(B.s);
@@ -1506,8 +1415,11 @@ static int32_t load_flat(FILE* f, u64 file_bytes, const dbsp_schema& sc, u64 kin
     bld.push(row, row + sc.n_key_lanes, w[i]);
     memcpy(prev, row, sizeof(row));
   }
-  CHECK_ARG(!(inv || dup || zero), "spine_load: rows of a batch are not consolidated (" + std::to_string(inv) + " out of order, " +
-                                       std::to_string(dup) + " duplicates, " + std::to_string(zero) + " zero weights)");
+  if (inv || dup || zero) {
+    g_err = "spine_load: rows of a batch are not consolidated (" + std::to_string(inv) + " out of order, " + std::to_string(dup) +
+            " duplicates, " + std::to_string(zero) + " zero weights)";
+    return DBSP_ERR_INVALID;
+  }
   *out = bld.done();
   return DBSP_OK;
 }
@@ -1586,16 +1498,14 @@ int32_t orc_spine_load(orc_ctx* c, const char* path, orc_spine** out) {
 // the multi-worker CPU runs use the in-process exchange of oracle/nexmark_workers.cpp / thread_workers.py.
 int32_t orc_comm_create(orc_ctx* c, int32_t rank, int32_t world, u64, uint8_t* blob) {
   NOT_NULL(c, "ctx");
-  CHECK_ARG(blob != nullptr, "comm_create: blob_out is NULL");
-  CHECK_ARG(world >= 1 && world <= DBSP_COMM_MAX_RANKS, "comm_create: world = " + std::to_string(world) + ": 1..32 ranks");
-  CHECK_ARG(rank >= 0 && rank < world, "comm_create: rank = " + std::to_string(rank) + " is not below world = " + std::to_string(world));
+  REFUSE(dv::check_comm_create(rank, world, blob));
   if (world != 1 || rank != 0) { g_err = "oracle: single worker only"; return DBSP_ERR_UNSUPPORTED; }
   if (blob) memset(blob, 0, DBSP_COMM_BLOB_BYTES);
   return DBSP_OK;
 }
 int32_t orc_comm_connect(orc_ctx* c, const uint8_t* blobs) {
   NOT_NULL(c, "ctx");
-  CHECK_ARG(blobs != nullptr, "comm_connect: blobs is NULL");
+  NOT_NULL(blobs, "blobs");
   return DBSP_OK;
 }
 int32_t orc_comm_destroy(orc_ctx* c) { NOT_NULL(c, "ctx"); return DBSP_OK; }
@@ -1625,9 +1535,7 @@ int32_t orc_shard2(orc_ctx* c, const orc_batch* a, const orc_batch* b, orc_batch
 }
 int32_t orc_gather(orc_ctx* c, const orc_batch* b, int32_t root, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
-  CHECK_ARG(root == 0, "gather: root = " + std::to_string(root) + " is not a rank of a group of 1");
+  REFUSE(dv::check_gather(out, S(b), root, 1));
   *out = wrap(b->p);
   return DBSP_OK;
 }

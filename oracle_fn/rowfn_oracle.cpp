@@ -104,22 +104,10 @@ void join_into_fn(const Batch& L, const Batch& R, const dbsp_rowfn& f, bool swap
   }
 }
 
-// A fan-out of n rows into n * n_out rows before consolidation: the CUDA library's 32-bit bound, from the sizes.
-#define FANOUT_ROWS(n, n_out, what)                                                   \
-  do {                                                                                \
-    const std::string m__ = dv::valid_fanout_rows((n), (n_out), (what));              \
-    if (!m__.empty()) { g_err = m__; return DBSP_ERR_UNSUPPORTED; }                   \
-  } while (0)
-
 // n_out == 0: a plain row function (`_fn`); otherwise a fan-out whose program runs for j = 0 .. n_out-1 per row.
-int32_t table_to_batch_fn(const char* what, const u64* const* cols, uint32_t ncols, unsigned col_mask, const i64* w, u64 n,
-                          const dbsp_rowfn* fn, orc_batch** out, uint32_t n_out = 0) {
-  REFUSE(dv::valid_rowfn(fn, (int)ncols, (int)ncols, (int)ncols, what, n_out != 0 ? dv::SRC_BIT_FANOUT : 0u));
+int32_t table_to_batch_fn(const u64* const* cols, uint32_t ncols, const i64* w, u64 n, const dbsp_rowfn* fn, orc_batch** out,
+                          uint32_t n_out = 0) {
   const unsigned used = dv::rowfn_table_mask(*fn);
-  CHECK_ARG((used & ~col_mask) == 0, std::string(what) + ": fn reads column " + std::to_string(__builtin_ctz((used & ~col_mask) | 0x100u)) +
-                                         ", which col_mask left out of the upload");
-  REFUSE(valid_cols(what, cols, (int)ncols, n, used));
-  FANOUT_ROWS(n, n_out, what);
   Tuples t(fn->out_schema);
   u64 lv[MAXL] = {0}, row[MAXL];
   for (u64 i = 0; i < n; i++) {
@@ -130,11 +118,6 @@ int32_t table_to_batch_fn(const char* what, const u64* const* cols, uint32_t nco
   }
   *out = wrap(t.build());
   return DBSP_OK;
-}
-
-std::string valid_join_fn(const char* what, const dbsp_schema& left, const dbsp_schema& right, const dbsp_rowfn* f) {
-  if (!dv::same_key_lanes(left, right)) return std::string(what) + ": the two inputs differ in key lanes (count or type)";
-  return dv::valid_rowfn(f, left.n_key_lanes, left.n_val_lanes, right.n_val_lanes, what);
 }
 
 // Upsert::eval for one key (operator/upsert.rs:161-208): retract the key's current values in the output trace, insert
@@ -171,41 +154,30 @@ extern "C" {
 int32_t orc_batch_from_table_fn(orc_ctx* c, const u64* const* cols, uint32_t ncols, const i64* w, u64 n, int32_t,
                                 const dbsp_rowfn* fn, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  CHECK_ARG(ncols >= 1 && ncols <= MAXL, "batch_from_table_fn: n_cols = " + std::to_string(ncols) + ": a table has 1..8 columns");
-  ROWS32(n);
-  return table_to_batch_fn(WHAT, cols, ncols, ~0u, w, n, fn, out);
+  REFUSE(dv::check_table(WHAT, out, cols, ncols, n, fn));
+  return table_to_batch_fn(cols, ncols, w, n, fn, out);
 }
 
 int32_t orc_batch_from_upload_fn(orc_ctx* c, orc_upload* u, const dbsp_rowfn* fn, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(u, "upload");
-  return table_to_batch_fn(WHAT, u->cols, u->n_cols, u->col_mask, u->w, u->n, fn, out);
+  REFUSE(dv::check_upload(WHAT, out, upload_of(u, c), fn));
+  return table_to_batch_fn(u->cols, u->n_cols, u->w, u->n, fn, out);
 }
 
-uint32_t orc_rowfn_table_mask(const dbsp_rowfn* fn) {
-  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "rowfn_table_mask").empty()) return 0;
-  return dv::rowfn_table_mask(*fn);
-}
+uint32_t orc_rowfn_table_mask(const dbsp_rowfn* fn) { return dv::checked_table_mask(fn, WHAT); }
 
 // flat_map_index over a raw table with a fan-out (filter_map.rs:124-160: the closure returns an iterator).
 int32_t orc_batch_from_table_fanout(orc_ctx* c, const u64* const* cols, uint32_t ncols, const i64* w, u64 n, int32_t,
                                     const dbsp_rowfn* fn, uint32_t n_out, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  CHECK_ARG(ncols >= 1 && ncols <= MAXL, "batch_from_table_fanout: n_cols = " + std::to_string(ncols) + ": a table has 1..8 columns");
-  REFUSE(dv::valid_fanout(n_out, WHAT));
-  ROWS32(n);
-  return table_to_batch_fn(WHAT, cols, ncols, ~0u, w, n, fn, out, n_out);
+  REFUSE(dv::check_table(WHAT, out, cols, ncols, n, fn, n_out));
+  return table_to_batch_fn(cols, ncols, w, n, fn, out, n_out);
 }
 
 int32_t orc_batch_from_upload_fanout(orc_ctx* c, orc_upload* u, const dbsp_rowfn* fn, uint32_t n_out, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(u, "upload");
-  REFUSE(dv::valid_fanout(n_out, WHAT));
-  return table_to_batch_fn(WHAT, u->cols, u->n_cols, u->col_mask, u->w, u->n, fn, out, n_out);
+  REFUSE(dv::check_upload(WHAT, out, upload_of(u, c), fn, n_out));
+  return table_to_batch_fn(u->cols, u->n_cols, u->w, u->n, fn, out, n_out);
 }
 
 // antijoin (operator/join.rs:294-320) incrementally, as the formula reads: a delta row (k, v1, w) with N(k) distinct
@@ -214,12 +186,7 @@ int32_t orc_batch_from_upload_fanout(orc_ctx* c, orc_upload* u, const dbsp_rowfn
 int32_t orc_antijoin_delta(orc_ctx* c, const orc_batch* delta, const orc_spine* tr, const orc_batch* kd,
                            const orc_spine* kt, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(delta, "delta");
-  NOT_NULL(tr, "trace");
-  NOT_NULL(kd, "key_delta");
-  NOT_NULL(kt, "key_trace");
-  REFUSE(dv::valid_antijoin(delta->p->s, tr->s.s, kd->p->s, kt->s.s));
+  REFUSE(dv::valid_antijoin(out, S(delta), S(tr), S(kd), S(kt)));
   const Batch& D = *delta->p;
   const int nk = D.s.n_key_lanes;
   Tuples t(D.s);
@@ -262,11 +229,7 @@ int32_t orc_antijoin_delta(orc_ctx* c, const orc_batch* delta, const orc_spine* 
 int32_t orc_aggregate_fold(orc_ctx* c, const orc_batch* delta, const orc_spine* in_tr, const orc_spine* out_tr,
                            const dbsp_fold* fold, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(delta, "delta");
-  NOT_NULL(in_tr, "in_trace");
-  NOT_NULL(out_tr, "out_trace");
-  REFUSE(dv::valid_fold(delta->p->s, in_tr->s.s, out_tr->s.s, fold));
+  REFUSE(dv::valid_fold(out, S(delta), S(in_tr), S(out_tr), fold));
   const Batch& D = *delta->p;
   const int n_acc = fold->n_acc, nov = out_tr->s.s.n_val_lanes;
   const dbsp_rowfn step = dv::fold_step_rowfn(*fold);
@@ -300,11 +263,8 @@ int32_t orc_aggregate_fold(orc_ctx* c, const orc_batch* delta, const orc_spine* 
 int32_t orc_upsert_commands(orc_ctx* c, const dbsp_schema* table, const u64* const* cols, const uint8_t* insert, u64 n,
                             u64 seq0, int32_t, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  REFUSE(dv::valid_upsert(table, n, seq0));
+  REFUSE(dv::valid_upsert(out, table, cols, n, seq0));
   const int nk = table->n_key_lanes, nv = table->n_val_lanes;
-  REFUSE(valid_cols(WHAT, cols, nk + nv, n));
-  ROWS32(n);
   Tuples t(dv::upsert_command_schema(*table));
   u64 row[MAXL];
   for (u64 i = 0; i < n; i++) {
@@ -324,10 +284,7 @@ int32_t orc_upsert_commands(orc_ctx* c, const dbsp_schema* table, const u64* con
 // compactions.
 int32_t orc_upsert_delta(orc_ctx* c, const orc_batch* cmds, const orc_spine* table, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(cmds, "cmds");
-  NOT_NULL(table, "table");
-  REFUSE(dv::valid_upsert(cmds->p->s, table->s.s));
+  REFUSE(dv::valid_upsert(out, S(cmds), S(table)));
   const Batch& C = *cmds->p;
   const dbsp_schema& ts = table->s.s;
   // the commands: row j of the batch, its key at kof[j], its command word in value lane 0, its values after it
@@ -351,19 +308,13 @@ int32_t orc_upsert_delta(orc_ctx* c, const orc_batch* cmds, const orc_spine* tab
   return DBSP_OK;
 }
 
-uint32_t orc_fanout_table_mask(const dbsp_rowfn* fn) {
-  if (!dv::valid_rowfn(fn, MAXL, MAXL, MAXL, "fanout_table_mask", dv::SRC_BIT_FANOUT).empty()) return 0;
-  return dv::rowfn_table_mask(*fn);
-}
+uint32_t orc_fanout_table_mask(const dbsp_rowfn* fn) { return dv::checked_table_mask(fn, WHAT, dv::SRC_BIT_FANOUT); }
 
 // JoinTrace::eval with Time = () (operator/join.rs:732-863): delta joined with every batch of the trace.
 int32_t orc_join_delta_trace_fn(orc_ctx* c, const orc_batch* delta, const orc_spine* tr, const dbsp_rowfn* fn,
                                 int32_t delta_is_left, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(delta, "delta");
-  NOT_NULL(tr, "trace");
-  REFUSE(delta_is_left ? valid_join_fn(WHAT, delta->p->s, tr->s.s, fn) : valid_join_fn(WHAT, tr->s.s, delta->p->s, fn));
+  REFUSE(dv::check_join(WHAT, out, S(delta), S(tr), delta_is_left, fn));
   Tuples t(fn->out_schema);
   for (auto& b : tr->s.batches) join_into_fn(*delta->p, *b, *fn, !delta_is_left, t);
   *out = wrap(t.build());
@@ -372,10 +323,7 @@ int32_t orc_join_delta_trace_fn(orc_ctx* c, const orc_batch* delta, const orc_sp
 
 int32_t orc_join_batches_fn(orc_ctx* c, const orc_batch* l, const orc_batch* r, const dbsp_rowfn* fn, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(l, "left");
-  NOT_NULL(r, "right");
-  REFUSE(valid_join_fn(WHAT, l->p->s, r->p->s, fn));
+  REFUSE(dv::check_join(WHAT, out, S(l), S(r), fn));
   Tuples t(fn->out_schema);
   join_into_fn(*l->p, *r->p, *fn, false, t);
   *out = wrap(t.build());
@@ -386,14 +334,8 @@ int32_t orc_join_batches_fn(orc_ctx* c, const orc_batch* l, const orc_batch* r, 
 // the sum, nor (WEIGH_AVG) to the count.
 int32_t orc_weigh_fn(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* f, int32_t mode, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
+  REFUSE(dv::check_weigh(out, S(b), f, mode));
   const Batch& B = *b->p;
-  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || mode == DBSP_WEIGH_AVG, "weigh_fn: mode = " + std::to_string(mode) + " is not a weigh mode");
-  CHECK_ARG(mode == DBSP_WEIGH_LINEAR || B.s.n_key_lanes < MAXL, "weigh_fn: WEIGH_AVG adds a key lane and the batch already has 8");
-  CHECK_ARG(mode == DBSP_WEIGH_AVG || B.s.n_key_lanes >= 1, "weigh_fn: WEIGH_LINEAR of a batch without key lanes has no output lanes");
-  REFUSE(dv::valid_rowfn(f, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, WHAT));
-  CHECK_ARG(f->out_schema.n_key_lanes + f->out_schema.n_val_lanes == 1, "weigh_fn: fn.out_schema must have one lane (the factor)");
   dbsp_schema s = B.s;
   s.n_val_lanes = 0;
   if (mode == DBSP_WEIGH_AVG) { s.lane_types[s.n_key_lanes] = DBSP_U64; s.n_key_lanes++; }
@@ -423,10 +365,8 @@ int32_t orc_weigh_fn(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* f, int32_
 }
 
 // Map/FlatMap/Index::eval + from_tuples (operator/filter_map.rs:563-577,700-724); n_out == 0: no fan-out.
-static int32_t map_index_fn(const char* what, const orc_batch* b, const dbsp_rowfn* fn, uint32_t n_out, orc_batch** out) {
+static int32_t map_index_fn(const orc_batch* b, const dbsp_rowfn* fn, uint32_t n_out, orc_batch** out) {
   const Batch& B = *b->p;
-  REFUSE(dv::valid_rowfn(fn, B.s.n_key_lanes, B.s.n_val_lanes, B.s.n_val_lanes, what, n_out != 0 ? dv::SRC_BIT_FANOUT : 0u));
-  FANOUT_ROWS(B.indexed() ? B.V.n : B.K.n, n_out, what);
   Tuples t(fn->out_schema);
   u64 key[MAXL], val[MAXL] = {0}, row[MAXL];
   for (size_t k = 0; k < B.K.n; k++) {
@@ -446,18 +386,15 @@ static int32_t map_index_fn(const char* what, const orc_batch* b, const dbsp_row
 
 int32_t orc_map_index_fn(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* fn, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
-  return map_index_fn(WHAT, b, fn, 0, out);
+  REFUSE(dv::check_map_index(WHAT, out, S(b), fn));
+  return map_index_fn(b, fn, 0, out);
 }
 
 // flat_map / flat_map_index of a batch with a fan-out: j = 0 .. n_out-1 per row, in one pass.
 int32_t orc_map_index_fanout(orc_ctx* c, const orc_batch* b, const dbsp_rowfn* fn, uint32_t n_out, orc_batch** out) {
   NOT_NULL(c, "ctx");
-  NOT_NULL(out, "out");
-  NOT_NULL(b, "batch");
-  REFUSE(dv::valid_fanout(n_out, WHAT));
-  return map_index_fn(WHAT, b, fn, n_out, out);
+  REFUSE(dv::check_map_index(WHAT, out, S(b), b ? b->p->len() : 0, fn, n_out));
+  return map_index_fn(b, fn, n_out, out);
 }
 
 }  // extern "C"

@@ -5,12 +5,12 @@ include/dbsp_b200.h (CUDA library `libdbsp_b200.so`, sm_90a).  Importable as
 `dbsp_b200` through the shim at the repository root.
 """
 from . import _capi as capi
-from .circuit import Fold, FoldCount, FoldSum, Max, Min, RootCircuit, Stream, UpsertHandle
-from .zset import (Backend, Batch, Batcher, Merger, Proj, Schema, Spine, acc, col, const, fanout_index, key, lval, rval,
+from .circuit import Fold, FoldCount, FoldSum, Linear, Max, Min, RootCircuit, Stream, UpsertHandle
+from .zset import (After, Backend, Batch, Batcher, Before, Merger, Proj, RelRange, Schema, Spine, acc, col, const, fanout_index, key, lval, rval,
                    val, weight, where_)
 
 __all__ = [
     "capi", "RootCircuit", "Stream", "UpsertHandle", "Max", "Min", "FoldCount", "FoldSum", "Fold", "Backend", "Batch", "Proj",
     "Schema", "Spine", "Batcher", "Merger", "key", "lval", "rval", "val", "col", "const", "where_",
-    "fanout_index", "acc", "weight",
+    "fanout_index", "acc", "weight", "Linear", "Before", "After", "RelRange",
 ]

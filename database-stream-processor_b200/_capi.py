@@ -26,6 +26,7 @@ OP_COPY, OP_NEG, OP_ADD, OP_SUB, OP_MUL, OP_DIV = range(6)
 CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_IN = range(7)
 AGG_MAX, AGG_MIN, AGG_FOLD_COUNT, AGG_FOLD_SUM, AGG_WCOUNT, AGG_WCOUNT2 = range(6)
 WEIGH_LINEAR, WEIGH_AVG = 0, 1
+ROLLING_LINEAR, ROLLING_MAX, ROLLING_MIN = 0, 1, 2
 (FN_PUSH, FN_NEG, FN_ABS, FN_BNOT, FN_LNOT, FN_ADD, FN_SUB, FN_MUL, FN_DIV, FN_REM, FN_DIVU, FN_REMU, FN_MIN, FN_MAX,
  FN_MINU, FN_MAXU, FN_AND, FN_OR, FN_XOR, FN_SHL, FN_SHR, FN_SAR, FN_EQ, FN_NE, FN_LT, FN_LE, FN_GT, FN_GE, FN_LTU,
  FN_LEU, FN_GTU, FN_GEU, FN_IN, FN_SELECT) = range(34)
@@ -68,6 +69,11 @@ class CRowFn(C.Structure):
 class CFold(C.Structure):
     _fields_ = [("n_acc", C.c_uint8), ("n_step", C.c_uint8), ("pad_", C.c_uint8 * 6), ("init", C.c_uint64 * MAX_ACC),
                 ("step", CInsn * MAX_INSNS), ("output", CRowFn)]
+
+
+class CRelRange(C.Structure):
+    _fields_ = [("from_after", C.c_uint8), ("to_after", C.c_uint8), ("pad_", C.c_uint8 * 6), ("from_off", C.c_uint64),
+                ("to_off", C.c_uint64)]
 
 
 class DbspError(RuntimeError):
@@ -143,6 +149,7 @@ _SIGS = {
     "aggregate_fold": [_P, _P, _P, _P, C.POINTER(CFold), _PP],
     "upsert_commands": [_P, C.POINTER(CSchema), _PP, _P, C.c_uint64, C.c_uint64, C.c_int32, _PP],
     "upsert_delta": [_P, _P, _P, _PP],
+    "rolling_aggregate": [_P, _P, _P, _P, C.POINTER(CRelRange), C.c_int32, C.POINTER(CRowFn), _PP],
     "weigh": [_P, _P, C.POINTER(CExpr), C.c_int32, _PP],
     "weigh_fn": [_P, _P, C.POINTER(CRowFn), C.c_int32, _PP],
     "distinct_delta": [_P, _P, _P, _PP],
@@ -170,7 +177,7 @@ ROWFN_CALLS = {"batch_from_table_fn", "batch_from_upload_fn", "join_delta_trace_
                "map_index_fn", "batch_from_table_fanout", "batch_from_upload_fanout", "map_index_fanout"}
 # Operators added after that oracle: the CUDA library and the row-function oracle export them, the dbsp_proj oracle
 # does not.  `CApi.exports` tells a caller which of them a library has.
-LATER_CALLS = {"antijoin_delta", "aggregate_fold", "upsert_commands", "upsert_delta"}
+LATER_CALLS = {"antijoin_delta", "aggregate_fold", "upsert_commands", "upsert_delta", "rolling_aggregate"}
 
 
 class CApi:

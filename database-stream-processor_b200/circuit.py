@@ -18,8 +18,8 @@ from typing import Callable, Sequence
 import numpy as np
 
 from . import _capi as capi
-from .zset import (Backend, Batch, Expr, Fn, Pred, Proj, Schema, Spine, Src, acc, compile_fold, compile_fold_step, const, key,
-                   lval, rval, upsert_command_schema)
+from .zset import (After, Backend, Batch, Before, Expr, Fn, Pred, Proj, RelRange, Schema, Spine, Src, acc, compile_fold,
+                   compile_fold_step, const, key, lval, rval, upsert_command_schema)
 
 
 class Max:  # operator/aggregate/max.rs:36-55
@@ -64,6 +64,32 @@ class Fold:
             raise ValueError("Fold: the output is a fan-out closure; a key has one output")
         self.init, self.step, self.where, self.output = init, list(step), where, output
         self._c = compile_fold(init, code, output._c if output.is_fn else output.as_rowfn()._c)
+
+
+class Linear:
+    """The linear rolling aggregator (rolling_aggregate.rs LinearAggregator): per output lane of `f`, the sum of
+    f(pk, v) * weight over the window, wrapping in i64.  `f` is a Proj with value lanes only over key(i) (the partition
+    key), lval(i) / val(i) (the lanes after the timestamp) and constants; a row its filter drops adds 0."""
+
+    kind = capi.ROLLING_LINEAR
+
+    def __init__(self, f: Proj):
+        if f.schema.nk != 0 or f.schema.nv == 0:
+            raise ValueError(f"Linear: f must have value lanes only, has schema {f.schema}")
+        if f.is_fanout:
+            raise ValueError("Linear: f is a fan-out closure; a row has one term")
+        self.f = f
+
+
+def _rolling_kind(aggregator):
+    """(kind, f) of a rolling aggregator: Max, Min or Linear(f)"""
+    if isinstance(aggregator, Linear):
+        return capi.ROLLING_LINEAR, aggregator.f
+    if aggregator is Max or isinstance(aggregator, Max):
+        return capi.ROLLING_MAX, None
+    if aggregator is Min or isinstance(aggregator, Min):
+        return capi.ROLLING_MIN, None
+    raise ValueError(f"partitioned_rolling_aggregate: {aggregator!r} is not Max, Min or Linear(f)")
 
 
 class _KeyCounts:
@@ -780,6 +806,81 @@ class Stream:
             return st["wm"]
 
         return self._unary(fn, "watermark_monotonic", None)
+
+    # -- time series ---------------------------------------------------------
+    def partitioned_rolling_aggregate(self, aggregator, rng: RelRange) -> "Stream":
+        """partitioned_rolling_aggregate (operator/time_series/rolling_aggregate.rs:235-249): the stream is indexed by
+        the partition key PK, value lane 0 is the timestamp TS and the other value lanes are V.  For every (pk, ts)
+        with a row of positive weight, the output holds (pk, (ts, some, agg..)): `agg` aggregates the partition's rows
+        whose ts' lies in rng.range_of(ts), `some` is 0 (and agg 0) when none does.  `aggregator` is Max, Min (over V)
+        or Linear(f).  The stream is sharded by PK first.  The operator's traces are the stream's `rolling_in_trace` and
+        `rolling_out_trace`."""
+        return self._rolling(self, aggregator, rng)
+
+    def partitioned_rolling_aggregate_linear(self, f: Proj, rng: RelRange) -> "Stream":
+        """partitioned_rolling_aggregate_linear (rolling_aggregate.rs:367-385) = the rolling aggregate of Linear(f)."""
+        return self._rolling(self, Linear(f), rng)
+
+    def partitioned_rolling_aggregate_with_watermark(self, watermark: "Stream", partition: Proj, aggregator,
+                                                     rng: RelRange) -> "Stream":
+        """partitioned_rolling_aggregate_with_watermark (rolling_aggregate.rs:155-220): the stream is indexed by the
+        timestamp (one key lane) and `partition` maps its value to (pk.., v..) (its key lanes are PK, its value lanes
+        V).  The watermark bounds the state: the input is windowed to [lower, max), lower = the start of the range
+        [from - to, Before(0)] of the watermark, and the output trace drops times below lower after each step.  Both
+        traces and the window's are exposed on the result (`rolling_in_trace`, `rolling_out_trace`, `window_trace`),
+        and `rolling_lower()` is the current lower bound."""
+        if self.schema.nk != 1:
+            raise ValueError(f"partitioned_rolling_aggregate_with_watermark: the stream is indexed by the timestamp "
+                             f"alone, has {self.schema.nk} key lanes")
+        ts = self.schema.key
+        signed = ts == "i"
+        lo_ts, hi_ts = (-(1 << 63), (1 << 63) - 1) if signed else (0, (1 << 64) - 1)
+        shifted = RelRange(rng.frm.sub(rng.to, signed), Before(0))
+        st = {"lower": lo_ts}
+
+        def bounds(wm):
+            r = shifted.range_of(wm, signed)
+            st["lower"] = lo_ts if r is None else r[0]
+            return st["lower"], hi_ts
+
+        window = self.window(watermark.apply(bounds))
+        pnk = partition.schema.nk
+        by_pk = Proj(Schema(partition.schema.key, ts + partition.schema.val),
+                     partition.out[:pnk] + [key(0)] + partition.out[pnk:], partition.where)
+        out = self.map_index(by_pk)._rolling(window.map_index(by_pk), aggregator, rng, lambda: st["lower"])
+        out.window_trace = window.window_trace
+        out.rolling_lower = lambda: st["lower"]
+        return out
+
+    def _rolling(self, win: "Stream", aggregator, rng: RelRange, lower: Callable[[], int] | None = None) -> "Stream":
+        """PartitionedRollingAggregate (rolling_aggregate.rs:286-359): the delta is `self`, the input trace integrates
+        `win` (self, or its windowed form), the output trace holds the operator's past outputs; `lower`, when given,
+        truncates the output trace's times below it after each step."""
+        be = self.circuit.be
+        if not be.api.exports("rolling_aggregate"):
+            raise capi.DbspError(f"{be.api.prefix}rolling_aggregate: this library does not export it")
+        kind, f = _rolling_kind(aggregator)
+        s = self.schema
+        if s.nv == 0:
+            raise ValueError("partitioned_rolling_aggregate: the stream has no value lanes; value lane 0 is the timestamp")
+        agg = f.schema.val if f is not None else s.val[1:]
+        out_schema = Schema(s.key, s.val[0] + "u" + agg)
+        d = self.shard()
+        w = d if win is self else win.shard()
+        in_tr, out_tr = Spine(be, s), Spine(be, out_schema)
+
+        def fn(dd: Batch, wd: Batch):
+            in_tr.insert(wd)
+            out = be.rolling_aggregate(dd, in_tr, out_tr, rng, kind, f)
+            out_tr.insert(out)
+            if lower is not None:
+                out_tr.truncate_values_below([lower()] + [0] * (out_schema.nv - 1))
+            return out
+
+        node = Node(self.circuit, [d.node, w.node], fn, "partitioned_rolling_aggregate")
+        out = Stream(self.circuit, node, out_schema, True)
+        out.rolling_in_trace, out.rolling_out_trace = in_tr, out_tr
+        return out
 
     # -- communication -------------------------------------------------------
     def shard(self) -> "Stream":

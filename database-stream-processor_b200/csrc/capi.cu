@@ -1259,6 +1259,10 @@ int32_t dbsp_aggregate_fold(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine
                             const dbsp_fold* fold, dbsp_batch** out) { ENTER(ctx);
   REFUSE(dv::valid_fold(out, S(d), S(in_tr), S(out_tr), fold));
   OUT1(op_aggregate_fold(ctx, B(d), in_tr, out_tr, fold, &o__)) }
+int32_t dbsp_rolling_aggregate(dbsp_ctx* ctx, const dbsp_batch* d, const dbsp_spine* in_tr, const dbsp_spine* out_tr,
+                               const dbsp_rel_range* range, int32_t kind, const dbsp_rowfn* f, dbsp_batch** out) { ENTER(ctx);
+  REFUSE(dv::valid_rolling(out, S(d), S(in_tr), S(out_tr), range, kind, f));
+  OUT1(op_rolling_aggregate(ctx, B(d), in_tr, out_tr, *range, kind, f, &o__)) }
 int32_t dbsp_upsert_commands(dbsp_ctx* ctx, const dbsp_schema* table, const uint64_t* const* cols,
                              const uint8_t* insert, uint64_t n, uint64_t seq0, int32_t on_device,
                              dbsp_batch** out) { ENTER(ctx);

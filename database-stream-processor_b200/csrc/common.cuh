@@ -116,7 +116,7 @@ struct Spine {
 // stream; bench.py's roofline figures come from here).
 enum KernelId {
   KID_MERGE = 0, KID_MERGE_PARTITION, KID_PROBE_RANGES, KID_PROBE_FILL, KID_PROJECT, KID_RADIX_SORT, KID_PACK,
-  KID_HEADS, KID_EMIT, KID_MINMAX, KID_SEG_REDUCE, KID_LOOKUP, KID_COMPACT, KID_SCAN, KID_AGG_PICK, KID_MISC, KID_SHARD, KID_CHUNK_SORT, KID_ANTIJOIN, KID_AGG_FOLD, KID_UPSERT,
+  KID_HEADS, KID_EMIT, KID_MINMAX, KID_SEG_REDUCE, KID_LOOKUP, KID_COMPACT, KID_SCAN, KID_AGG_PICK, KID_MISC, KID_SHARD, KID_CHUNK_SORT, KID_ANTIJOIN, KID_AGG_FOLD, KID_UPSERT, KID_ROLLING,
   KID_COUNT
 };
 struct ProfRec {

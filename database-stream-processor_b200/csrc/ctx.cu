@@ -26,7 +26,7 @@ const char* get_error() { return g_err.c_str(); }
 static const char* KNAMES[KID_COUNT] = {
     "merge_tiles", "merge_partition", "probe_ranges", "probe_fill", "project_rows", "radix_sort", "pack_keys",
     "heads", "emit", "minmax", "seg_reduce", "lookup", "compact", "scan", "agg_pick", "misc", "shard_scatter", "chunk_sort",
-    "antijoin_scale", "agg_fold", "upsert"};
+    "antijoin_scale", "agg_fold", "upsert", "rolling"};
 const char* kernel_name(int id) { return (id >= 0 && id < KID_COUNT) ? KNAMES[id] : "?"; }
 
 ProfScope::ProfScope(Ctx* ctx, int id, u64 bytes) : c(ctx) {

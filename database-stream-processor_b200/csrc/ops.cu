@@ -1,6 +1,8 @@
 // ops.cu — operator kernels: projection/filter, delta-vs-trace probes (join,
 // aggregate, distinct), window ranges, shard partition.  Each host entry
 // cites the reference `eval` it replaces (paths under crates/dbsp/src/).
+#include <cub/device/device_scan.cuh>
+
 #include "ops.cuh"
 #include "validate.h"
 
@@ -1025,6 +1027,263 @@ __global__ void k_shard_scatter(Cols in, int L, const i64* w, const u32* flags, 
   }
 }
 
+// ---------------- rolling aggregates (time_series/rolling_aggregate.rs) --------------------------------------------
+// Rows are (PK lanes, TS, ...); every kernel below compares the first nk + 1 lanes, flipped like the batch.  TS
+// arithmetic is range.rs's, in TS's type (u64, or i64 when sgn): `ts_add` / `ts_sub` are the checked forms (false on
+// overflow), `sat_*` the saturating ones.  The offsets of an i64 TS are at most INT64_MAX (validate.h).
+struct RollArgs {
+  u64 from_off, to_off;
+  int from_after, to_after, sgn;
+};
+__device__ __forceinline__ bool ts_add(u64 x, u64 off, int sgn, u64* r) {
+  if (!sgn) { *r = x + off; return *r >= x; }
+  if ((i64)x > INT64_MAX - (i64)off) return false;
+  *r = (u64)((i64)x + (i64)off);
+  return true;
+}
+__device__ __forceinline__ bool ts_sub(u64 x, u64 off, int sgn, u64* r) {
+  if (!sgn) { *r = x - off; return x >= off; }
+  if ((i64)x < INT64_MIN + (i64)off) return false;
+  *r = (u64)((i64)x - (i64)off);
+  return true;
+}
+__device__ __forceinline__ u64 sat_add(u64 x, u64 off, int sgn) {
+  u64 r;
+  return ts_add(x, off, sgn, &r) ? r : sgn ? (u64)INT64_MAX : ~0ull;
+}
+__device__ __forceinline__ u64 sat_sub(u64 x, u64 off, int sgn) {
+  u64 r;
+  return ts_sub(x, off, sgn, &r) ? r : sgn ? (u64)INT64_MIN : 0ull;
+}
+// RelRange::range_of (range.rs): false when the range lies outside TS
+__device__ __forceinline__ bool range_of(const RollArgs& a, u64 ts, u64* lo, u64* hi) {
+  if (a.from_after) { if (!ts_add(ts, a.from_off, a.sgn, lo)) return false; }
+  else *lo = sat_sub(ts, a.from_off, a.sgn);
+  if (a.to_after) *hi = sat_add(ts, a.to_off, a.sgn);
+  else if (!ts_sub(ts, a.to_off, a.sgn, hi)) return false;
+  return true;
+}
+// RelRange::affected_range_of (range.rs): the times whose range holds ts
+__device__ __forceinline__ bool affected_of(const RollArgs& a, u64 ts, u64* lo, u64* hi) {
+  if (a.to_after) *lo = sat_sub(ts, a.to_off, a.sgn);
+  else if (!ts_add(ts, a.to_off, a.sgn, lo)) return false;
+  if (a.from_after) { if (!ts_sub(ts, a.from_off, a.sgn, hi)) return false; }
+  else *hi = sat_add(ts, a.from_off, a.sgn);
+  return true;
+}
+// The TS rows to gather for the times [a, b]: the union of their ranges and [a, b] itself (whose rows decide
+// which times get an output), widened to a hull; both ends are monotone, so sorted intervals stay sorted.
+__device__ __forceinline__ u64 gather_lo(const RollArgs& r, u64 a) { return r.from_after ? a : sat_sub(a, r.from_off, r.sgn); }
+__device__ __forceinline__ u64 gather_hi(const RollArgs& r, u64 b) { return r.to_after ? sat_add(b, r.to_off, r.sgn) : b; }
+__device__ __forceinline__ bool same_lanes(const Cols& C, u64 i, u64 j, int nl) {
+  for (int l = 0; l < nl; l++)
+    if (C.c[l][i] != C.c[l][j]) return false;
+  return true;
+}
+
+// 1. Per distinct (pk, ts) of delta (rows 2i, 2i+1): [ts, ts] and affected_range_of(ts) as rows (pk, a, b) of weight
+// 1; every other slot gets weight 0, which the consolidation drops.
+__global__ void k_roll_intervals(Cols D, u64 n, int nk, RollArgs ra, MCols out, i64* out_w) {
+  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const u64 ts = D.c[nk][i];
+  const bool head = i == 0 || !same_lanes(D, i, i - 1, nk + 1);
+  u64 lo = ts, hi = ts;
+  const bool aff = head && affected_of(ra, ts, &lo, &hi);
+  for (int l = 0; l < nk; l++) out.c[l][2 * i] = out.c[l][2 * i + 1] = D.c[l][i];
+  out.c[nk][2 * i] = out.c[nk + 1][2 * i] = ts;
+  out.c[nk][2 * i + 1] = lo;
+  out.c[nk + 1][2 * i + 1] = hi;
+  out_w[2 * i] = head ? 1 : 0;
+  out_w[2 * i + 1] = aff ? 1 : 0;
+}
+// The segmented max-scan of the interval ends (flipped), restarting at each partition: an interval list sorted by
+// (pk, a) then covers ts iff ts <= the scanned end of the last interval with a <= ts.
+struct SegMax {
+  u64 v;
+  u32 head;
+};
+struct SegMaxOp {
+  __device__ __forceinline__ SegMax operator()(const SegMax& a, const SegMax& b) const {
+    return SegMax{b.head ? b.v : max(a.v, b.v), a.head | b.head};
+  }
+};
+__global__ void k_roll_segs(Cols I, u64 n, int nk, u64 tflip, SegMax* s) {
+  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  s[i] = SegMax{I.c[nk + 1][i] ^ tflip, (i == 0 || !same_lanes(I, i, i - 1, nk)) ? 1u : 0u};
+}
+// 2a. Gather groups: an interval starts a new one when its partition changes or its gather window starts after the
+// hull of the windows before it.  flags[n] = 0 for the ordered compaction.
+__global__ void k_roll_groups(Cols I, const SegMax* bmax, u64 n, int nk, RollArgs ra, u64 tflip, u32* flags) {
+  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > n) return;
+  if (i == n) { flags[n] = 0; return; }
+  bool head = i == 0 || !same_lanes(I, i, i - 1, nk);
+  if (!head) head = (gather_lo(ra, I.c[nk][i]) ^ tflip) > (gather_hi(ra, bmax[i - 1].v ^ tflip) ^ tflip);
+  flags[i] = head ? 1u : 0u;
+}
+// group g = intervals [H[g], H[g+1]): its rows (pk.., lo, hi) of the TS rows to gather
+__global__ void k_roll_group_rows(Cols I, const SegMax* bmax, const u64* H, u64 m, int nk, RollArgs ra, u64 tflip, MCols W) {
+  u64 g = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= m) return;
+  const u64 h = H[g], e = H[g + 1] - 1;
+  for (int l = 0; l < nk; l++) W.c[l][g] = I.c[l][h];
+  W.c[nk][g] = gather_lo(ra, I.c[nk][h]);
+  W.c[nk + 1][g] = gather_hi(ra, bmax[e].v ^ tflip);
+}
+// 2b. Per (group g, batch b): the rows of batch b inside group g, by two binary searches; cnt[nb * m] = 0.
+__global__ void k_roll_range_bounds(Cols W, u64 m, BatchRefs tr, int nk, Flips f, u32* start, u32* cnt) {
+  u64 x = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  const u64 total = m * (u64)tr.nb;
+  if (x > total) return;
+  if (x == total) { cnt[total] = 0; return; }
+  const int b = (int)(x / m);
+  const u64 g = x - (u64)b * m;
+  u64 q[MAXL];
+  for (int l = 0; l < nk + 1; l++) q[l] = W.c[l][g] ^ f.f[l];
+  const Cols& T = tr.b[b].c;
+  const u64 s = lower_bound_q(T, 0, tr.b[b].n, q, nk + 1, f);
+  q[nk] = W.c[nk + 1][g] ^ f.f[nk];
+  const u64 e = upper_bound_q(T, s, tr.b[b].n, q, nk + 1, f);
+  start[x] = (u32)s;
+  cnt[x] = (u32)(e - s);
+}
+// the first output row of every batch's slices (pos[b * m], b = 0 .. nb; the last is the total), in one read-back
+__global__ void k_roll_publish(const u32* pos, u64 m, int nb, Mail mail) {
+  u64 v[MAX_REFS + 1];
+  for (int b = 0; b <= nb; b++) v[b] = pos[(u64)b * m];
+  mail_publish(mail, v, nb + 1);
+}
+// output row o: the (batch, group) slice holding it (the last slice starting at or before o), then a copy of the row
+__global__ void k_roll_range_copy(const u32* start, const u32* pos, u64 ns, BatchRefs tr, u64 m, int L, u64 total,
+                                  MCols out, i64* out_w) {
+  u64 o = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= total) return;
+  u64 lo = 0, hi = ns;   // largest x < ns with pos[x] <= o
+  while (hi - lo > 1) {
+    const u64 mid = (lo + hi) >> 1;
+    if (pos[mid] <= o) lo = mid; else hi = mid;
+  }
+  const int b = (int)(lo / m);
+  const u64 r = start[lo] + (o - pos[lo]);
+  for (int l = 0; l < L; l++) out.c[l][o] = tr.b[b].c.c[l][r];
+  out_w[o] = tr.b[b].w[r];
+}
+// whether (pk, ts) of row `row` of R lies in an affected interval of I (sorted by (pk, a), ends max-scanned)
+__device__ __forceinline__ bool roll_member(const Cols& I, const SegMax* bmax, u64 nI, const Cols& R, u64 row, int nk,
+                                            const Flips& f) {
+  u64 q[MAXL];
+  for (int l = 0; l < nk + 1; l++) q[l] = R.c[l][row] ^ f.f[l];
+  const u64 k = upper_bound_q(I, 0, nI, q, nk + 1, f);
+  if (k == 0) return false;
+  for (int l = 0; l < nk; l++)
+    if (I.c[l][k - 1] != R.c[l][row]) return false;
+  return q[nk] <= bmax[k - 1].v;
+}
+// 4. the old outputs at the affected times, negated (keep[n] = 0 for the ordered compaction)
+__global__ void k_roll_retract(Cols O, const i64* wO, u64 n, Cols I, const SegMax* bmax, u64 nI, int nk, Flips f,
+                               u32* keep, i64* neww) {
+  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > n) return;
+  if (i == n) { keep[n] = 0; return; }
+  keep[i] = roll_member(I, bmax, nI, O, i, nk, f) ? 1u : 0u;
+  neww[i] = (i64)((u64)0 - (u64)wO[i]);
+}
+// 3a. LINEAR: per gathered row, f(pk, v) * weight per output lane (0 for a row whose keep flag is 0), for the scan.
+// V is G's value lanes after TS, so G's columns are shifted for the row function's LVAL.
+__global__ void k_roll_terms(Cols V, const i64* w, u64 n, int nk, dbsp_rowfn fn, int n_agg, i64* terms) {
+  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  u64 st[DBSP_MAX_STACK];
+  run_rowfn(fn, ColEnv{V, nk, i}, st);
+  const bool keep = st[n_agg] != 0;
+  for (int l = 0; l < n_agg; l++) terms[(u64)l * n + i] = (i64)(keep ? st[l] * (u64)w[i] : 0);
+}
+// 3b. MAX / MIN: the better of two rows of G by their V lanes (lanes v0 .. v0 + nvv), ties to the first
+__device__ __forceinline__ u32 roll_better(const Cols& G, u32 i, u32 j, int v0, int nvv, const Flips& f, int is_max) {
+  for (int l = v0; l < v0 + nvv; l++) {
+    const u64 a = G.c[l][i] ^ f.f[l], b = G.c[l][j] ^ f.f[l];
+    if (a != b) return ((a > b) == (is_max != 0)) ? i : j;
+  }
+  return i;
+}
+constexpr int RMQ_BLK = 32;
+__device__ __forceinline__ u32 roll_scan(const Cols& G, u32 lo, u32 hi, int v0, int nvv, const Flips& f, int is_max) {
+  u32 best = lo;   // rows [lo, hi], lo <= hi
+  for (u32 r = lo + 1; r <= hi; r++) best = roll_better(G, best, r, v0, nvv, f, is_max);
+  return best;
+}
+// the sparse table's level 0: the best row of each 32-row block
+__global__ void k_roll_rmq_base(Cols G, u64 n, int v0, int nvv, Flips f, int is_max, u32* t0) {
+  u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j * RMQ_BLK >= n) return;
+  t0[j] = roll_scan(G, (u32)(j * RMQ_BLK), (u32)min(n - 1, j * RMQ_BLK + RMQ_BLK - 1), v0, nvv, f, is_max);
+}
+// level k from level k - 1: entry j covers blocks [j, j + 2^k)
+__global__ void k_roll_rmq_level(Cols G, const u32* prev, u32* cur, u64 nblk, u64 half, int v0, int nvv, Flips f,
+                                 int is_max) {
+  u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j + 2 * half > nblk) return;
+  cur[j] = roll_better(G, prev[j], prev[j + half], v0, nvv, f, is_max);
+}
+struct RollOut {
+  int kind, n_agg, nvv;
+  const i64* psum;   // LINEAR: n_agg prefix sums of n rows each
+  const u32* rmq;    // MAX / MIN: levels of nblk entries each
+  u64 nblk;
+};
+// 3. Per first row of a (pk, ts) group of G that is an affected time with a row of positive weight and a range: the
+// window's rows [l, r) in G by two binary searches, then its aggregate; out lanes (ts, some, agg..), keep[n] = 0.
+__global__ void k_roll_out(Cols G, const i64* wG, u64 n, Cols I, const SegMax* bmax, u64 nI, int nk, Flips f,
+                           RollArgs ra, RollOut ro, u32* keep, MCols out) {
+  u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > n) return;
+  if (i == n) { keep[n] = 0; return; }
+  keep[i] = 0;
+  if (i > 0 && same_lanes(G, i, i - 1, nk + 1)) return;
+  const u64 ts = G.c[nk][i];
+  u64 lo, hi;
+  if (!range_of(ra, ts, &lo, &hi) || !roll_member(I, bmax, nI, G, i, nk, f)) return;
+  bool pos = false;
+  for (u64 j = i; j < n && !pos && (j == i || same_lanes(G, j, i, nk + 1)); j++) pos = wG[j] > 0;
+  if (!pos) return;
+  u64 q[MAXL];
+  for (int l = 0; l < nk; l++) q[l] = G.c[l][i] ^ f.f[l];
+  q[nk] = lo ^ f.f[nk];
+  const u64 l0 = lower_bound_q(G, 0, n, q, nk + 1, f);
+  q[nk] = hi ^ f.f[nk];
+  const u64 r0 = upper_bound_q(G, l0, n, q, nk + 1, f);
+  const bool some = l0 < r0;
+  keep[i] = 1;
+  out.c[0][i] = ts;
+  out.c[1][i] = some ? 1 : 0;
+  if (ro.kind == DBSP_ROLLING_LINEAR) {
+    for (int l = 0; l < ro.n_agg; l++) {
+      const i64* p = ro.psum + (u64)l * n;
+      out.c[2 + l][i] = some ? (u64)p[r0 - 1] - (l0 ? (u64)p[l0 - 1] : 0ull) : 0ull;
+    }
+    return;
+  }
+  if (!some) {
+    for (int l = 0; l < ro.nvv; l++) out.c[2 + l][i] = 0;
+    return;
+  }
+  const int v0 = nk + 1, is_max = ro.kind == DBSP_ROLLING_MAX;
+  const u32 a = (u32)l0, b = (u32)(r0 - 1), ba = a / RMQ_BLK, bb = b / RMQ_BLK;
+  u32 best;
+  if (bb - ba <= 1) {
+    best = roll_scan(G, a, b, v0, ro.nvv, f, is_max);
+  } else {
+    best = roll_scan(G, a, (ba + 1) * RMQ_BLK - 1, v0, ro.nvv, f, is_max);
+    best = roll_better(G, best, roll_scan(G, bb * RMQ_BLK, b, v0, ro.nvv, f, is_max), v0, ro.nvv, f, is_max);
+    const u32 nb = bb - ba - 1, k = 31 - __clz(nb);   // blocks ba+1 .. bb-1: two overlapping entries of level k
+    const u32* t = ro.rmq + (u64)k * ro.nblk;
+    best = roll_better(G, best, roll_better(G, t[ba + 1], t[bb - (1u << k)], v0, ro.nvv, f, is_max), v0, ro.nvv, f, is_max);
+  }
+  for (int l = 0; l < ro.nvv; l++) out.c[2 + l][i] = G.c[v0 + l][best];
+}
+
 inline unsigned blocks(u64 n) { return (unsigned)((n + TB - 1) / TB); }
 // Row indices, offsets and scans of the operator kernels are 32-bit: reject (never wrap) anything larger.
 #define ROWS32(n, what)                                                                        \
@@ -1851,6 +2110,234 @@ int32_t op_window_delta(Ctx* ctx, const Spine* trace, const Batch* delta, int ha
   }
   if (rc != DBSP_OK) { for (Batch* b : parts) batch_unref(b); return rc; }
   return merge_tree(ctx, parts, s, out);
+}
+
+// A batch reference released at the end of a scope
+struct BatchHold {
+  Batch* b = nullptr;
+  ~BatchHold() { if (b) batch_unref(b); }
+};
+
+// The rows of `sp` inside the m groups W (lanes pk.., lo, hi: rows with that pk and lo <= TS <= hi), weights summed
+// over the spine's batches, zero sums dropped.  Per chunk of MAX_REFS batches: the slice bounds of every (batch, group)
+// by binary search, their scan, one read-back of every batch's first slot, one copy of the slices; each batch's
+// slices are a consolidated view in (pk, ts) order, and a merge tree unites the views.
+static int32_t roll_gather(Ctx* ctx, const Spine* sp, int nk, const Cols& W, u64 m, Batch** out) {
+  const dbsp_schema& s = sp->s;
+  const int L = s.n_key_lanes + s.n_val_lanes;
+  const size_t nbat = sp->batches.size();
+  std::vector<Batch*> parts;
+  auto fail = [&](int32_t rc) { for (Batch* p : parts) batch_unref(p); return rc; };
+  // slice starts, counts and their scan are u32: a chunk's rows (which bound its gathered rows) and its slice count
+  // stay below 2^32-1, else the call is refused
+  auto rows32 = [&](u64 v, const char* what) {
+    const dbsp_validate::Refusal r = dbsp_validate::valid_rows32(v, what);
+    if (r) set_error(r.text);
+    return r ? r.status : DBSP_OK;
+  };
+  for (size_t b0 = 0; m && b0 < nbat; b0 += MAX_REFS) {
+    BatchRefs refs;
+    refs.nb = (int)std::min<size_t>(MAX_REFS, nbat - b0);
+    u64 rows = 0;
+    for (int b = 0; b < refs.nb; b++) {
+      const Batch* t = sp->batches[b0 + b];
+      refs.b[b] = BatchRef{t->cols(), t->w, t->n};
+      rows += t->n;
+    }
+    if (rows == 0) continue;
+    const u64 ns = m * (u64)refs.nb;
+    int32_t rc = rows32(rows, "rolling_aggregate: the rows of 16 trace batches");
+    if (rc == DBSP_OK) rc = rows32(ns, "rolling_aggregate: groups x trace batches");
+    if (rc) return fail(rc);
+    BufP sb;
+    rc = dev_alloc(ctx, (size_t)(ns + 1) * 4 * 3, &sb);
+    if (rc) return fail(rc);
+    u32* start = (u32*)sb->p;
+    u32* cnt = start + (ns + 1);
+    u32* pos = cnt + (ns + 1);
+    const Flips f = sp->batches[b0]->flips();
+    {
+      u64 lg = 1; while ((1ull << lg) < rows / refs.nb + 1) lg++;
+      ProfScope ps(ctx, KID_ROLLING, m * (u64)(nk + 2) * 8 + ns * (2 * lg * (u64)(nk + 1) * 8 + 8));
+      k_roll_range_bounds<<<blocks(ns + 1), TB, 0, ctx->stream>>>(W, m, refs, nk, f, start, cnt);
+    }
+    LAUNCH_COUNT(ctx);
+    if ((rc = exclusive_scan_u32(ctx, cnt, pos, ns))) return fail(rc);
+    const Mail mail = mail_begin(ctx);
+    k_roll_publish<<<1, 1, 0, ctx->stream>>>(pos, m, refs.nb, mail);
+    LAUNCH_COUNT(ctx);
+    u64 first[MAX_REFS + 1];
+    if ((rc = mail_finish(ctx, mail, first, refs.nb + 1))) return fail(rc);
+    const u64 total = first[refs.nb];
+    if (total == 0) continue;
+    Batch* all;
+    MCols oc;
+    i64* ow;
+    if ((rc = batch_alloc(ctx, s, total, &all, &oc, &ow))) return fail(rc);
+    {
+      ProfScope ps(ctx, KID_ROLLING, total * (u64)(L + 1) * 8 * 2);
+      k_roll_range_copy<<<blocks(total), TB, 0, ctx->stream>>>(start, pos, ns, refs, m, L, total, oc, ow);
+    }
+    LAUNCH_COUNT(ctx);
+    for (int b = 0; b < refs.nb; b++)
+      if (first[b + 1] > first[b]) parts.push_back(batch_slice(ctx, all, first[b], first[b + 1]));
+    batch_unref(all);
+  }
+  return merge_tree(ctx, parts, s, out);
+}
+
+// PartitionedRollingAggregate::eval (operator/time_series/rolling_aggregate.rs:436-604) without the radix tree:
+// 1. the delta's affected intervals (affected_range_of(ts) and [ts, ts] per distinct (pk, ts)), sorted, their ends
+//    max-scanned per partition; 2. in_trace's rows of every time those intervals' windows can read (G); 3. per
+//    affected (pk, ts) of G with a positive row and a range, its window in G by binary search, aggregated from a
+//    prefix sum (LINEAR: wrapping i64 is a group) or a sparse table over 32-row blocks (MAX / MIN); 4. out_trace's
+//    rows at the affected times negated and merged with the new rows.  The work is the delta plus the rows the
+//    affected windows hold, never a whole partition.
+int32_t op_rolling_aggregate(Ctx* ctx, const Batch* delta, const Spine* in_tr, const Spine* out_tr,
+                             const dbsp_rel_range& range, int kind, const dbsp_rowfn* fn, Batch** out) {
+  cudaStream_t st = ctx->stream;
+  const dbsp_schema& os = out_tr->s;
+  const int nk = delta->s.n_key_lanes, nv = delta->s.n_val_lanes, n_agg = os.n_val_lanes - 2;
+  const u64 n = delta->n;
+  if (n == 0) { *out = batch_new_empty(ctx, os); return DBSP_OK; }
+  if (2 * n > (u64)INT32_MAX) {   // the intervals (two per delta row) are scanned with an int count
+    set_error("rolling_aggregate: n = " + std::to_string(n) + ": 2^30 or more delta rows in one call; split the delta");
+    return DBSP_ERR_UNSUPPORTED;
+  }
+  const Flips f = delta->flips();
+  const u64 tflip = f.f[nk];
+  const RollArgs ra{range.from_off, range.to_off, range.from_after ? 1 : 0, range.to_after ? 1 : 0,
+                    delta->s.lane_types[nk] == DBSP_I64 ? 1 : 0};
+  // 1. affected intervals (pk.., a, b), sorted by the consolidation
+  dbsp_schema is;
+  memset(&is, 0, sizeof(is));
+  is.n_key_lanes = (uint8_t)nk;
+  is.n_val_lanes = 2;
+  for (int l = 0; l < nk + 1; l++) is.lane_types[l] = delta->s.lane_types[l];
+  is.lane_types[nk + 1] = is.lane_types[nk];
+  BatchHold I;
+  {
+    TmpRows t;
+    TRY(tmp_alloc(ctx, nk + 2, 2 * n, &t));
+    {
+      ProfScope ps(ctx, KID_ROLLING, n * (u64)(nk + 1) * 8 + 2 * n * (u64)(nk + 3) * 8);
+      k_roll_intervals<<<blocks(n), TB, 0, st>>>(delta->cols(), n, nk, ra, t.c, t.w);
+    }
+    LAUNCH_COUNT(ctx);
+    TRY(consolidate_rows(ctx, is, t.cc(), t.w, 2 * n, &t.buf, &I.b));
+  }
+  const u64 nI = I.b->n;   // >= 1: every delta row has a head
+  BufP segb, tmpb;
+  TRY(dev_alloc(ctx, (size_t)nI * sizeof(SegMax) * 2, &segb));
+  SegMax* segs = (SegMax*)segb->p;
+  SegMax* bmax = segs + nI;
+  k_roll_segs<<<blocks(nI), TB, 0, st>>>(I.b->cols(), nI, nk, tflip, segs);
+  LAUNCH_COUNT(ctx);
+  size_t tmp_bytes = 0;
+  CUDA_TRY(cub::DeviceScan::InclusiveScan(nullptr, tmp_bytes, segs, bmax, SegMaxOp(), (int)nI, st));
+  TRY(dev_alloc(ctx, tmp_bytes, &tmpb));
+  CUDA_TRY(cub::DeviceScan::InclusiveScan(tmpb->p, tmp_bytes, segs, bmax, SegMaxOp(), (int)nI, st));
+  LAUNCH_COUNT(ctx);
+  // 2. gather groups: intervals whose gather windows overlap, merged
+  BufP gb, hb;
+  TRY(dev_alloc(ctx, (size_t)(nI + 1) * 4 * 2, &gb));
+  TRY(dev_alloc(ctx, (size_t)(nI + 1) * 8, &hb));
+  u32* gflag = (u32*)gb->p;
+  u32* gpos = gflag + (nI + 1);
+  u64* H = (u64*)hb->p;
+  k_roll_groups<<<blocks(nI + 1), TB, 0, st>>>(I.b->cols(), bmax, nI, nk, ra, tflip, gflag);
+  LAUNCH_COUNT(ctx);
+  const Mail gmail = mail_begin(ctx);
+  TRY(exclusive_scan_u32(ctx, gflag, gpos, nI, &gmail));
+  u64 m;
+  TRY(mail_finish(ctx, gmail, &m, 1));
+  k_scatter_index<<<blocks(nI), TB, 0, st>>>(gflag, gpos, nI, H, m);
+  LAUNCH_COUNT(ctx);
+  TmpRows W;
+  TRY(tmp_alloc(ctx, nk + 2, m, &W));
+  k_roll_group_rows<<<blocks(m), TB, 0, st>>>(I.b->cols(), bmax, H, m, nk, ra, tflip, W.c);
+  LAUNCH_COUNT(ctx);
+  BatchHold G;
+  TRY(roll_gather(ctx, in_tr, nk, W.cc(), m, &G.b));
+  // 3. the new rows (pk.., ts, some, agg..) with weight +1
+  BatchHold N;
+  const u64 ng = G.b->n;
+  if (ng == 0) {
+    N.b = batch_new_empty(ctx, os);
+  } else {
+    ROWS32(ng, "rolling_aggregate: gathered rows");
+    RollOut ro;
+    memset(&ro, 0, sizeof(ro));
+    ro.kind = kind;
+    ro.n_agg = n_agg;
+    ro.nvv = nv - 1;
+    const Cols g = G.b->cols();
+    BufP pb, rb;
+    if (kind == DBSP_ROLLING_LINEAR) {
+      Cols V = g;   // LVAL i = G's lane nk + 1 + i (V after TS)
+      for (int l = 0; l < nv - 1; l++) V.c[nk + l] = g.c[nk + 1 + l];
+      TRY(dev_alloc(ctx, (size_t)ng * 8 * 2 * n_agg, &pb));
+      i64* terms = (i64*)pb->p;
+      i64* psum = terms + (size_t)ng * n_agg;
+      {
+        ProfScope ps(ctx, KID_ROLLING, ng * (u64)(used_lanes(*fn, nk + nv - 1, nk) + 1) * 8 + ng * (u64)n_agg * 8);
+        k_roll_terms<<<blocks(ng), TB, 0, st>>>(V, G.b->w, ng, nk, *fn, n_agg, terms);
+      }
+      LAUNCH_COUNT(ctx);
+      for (int l = 0; l < n_agg; l++) TRY(inclusive_scan_i64(ctx, terms + (size_t)l * ng, psum + (size_t)l * ng, ng));
+      ro.psum = psum;
+    } else {
+      const u64 nblk = (ng + RMQ_BLK - 1) / RMQ_BLK;
+      int levels = 1;
+      while ((1ull << levels) <= nblk) levels++;
+      TRY(dev_alloc(ctx, (size_t)nblk * levels * 4, &rb));
+      u32* tab = (u32*)rb->p;
+      const int is_max = kind == DBSP_ROLLING_MAX;
+      {
+        // G's V lanes read once for the blocks; every level reads two entries and their rows' V lanes
+        ProfScope ps(ctx, KID_ROLLING, ng * (u64)(nv - 1) * 8 + (u64)levels * nblk * (4 + 2 * (u64)(nv - 1) * 8 + 8));
+        k_roll_rmq_base<<<blocks(nblk), TB, 0, st>>>(g, ng, nk + 1, nv - 1, G.b->flips(), is_max, tab);
+        LAUNCH_COUNT(ctx);
+        for (int k = 1; k < levels; k++) {
+          k_roll_rmq_level<<<blocks(nblk), TB, 0, st>>>(g, tab + (u64)(k - 1) * nblk, tab + (u64)k * nblk, nblk,
+                                                        1ull << (k - 1), nk + 1, nv - 1, G.b->flips(), is_max);
+          LAUNCH_COUNT(ctx);
+        }
+      }
+      ro.rmq = tab;
+      ro.nblk = nblk;
+    }
+    BufP kb;
+    TRY(dev_alloc(ctx, (size_t)(ng + 1) * 4, &kb));
+    TmpRows nvr;
+    TRY(tmp_alloc(ctx, 2 + n_agg, ng, &nvr));
+    {
+      // G's PK and TS lanes read for the heads and the searches; per output, its window's two ends (LINEAR) or up to
+      // 64 rows and two table entries (MAX / MIN), and its lanes written
+      const u64 per = kind == DBSP_ROLLING_LINEAR ? 2 * (u64)n_agg * 8 : (2 * RMQ_BLK + 2) * (u64)(nv - 1) * 8;
+      ProfScope ps(ctx, KID_ROLLING, ng * ((u64)(nk + 1) * 8 + 8) + ng * (per + (u64)(2 + n_agg) * 8));
+      k_roll_out<<<blocks(ng + 1), TB, 0, st>>>(g, G.b->w, ng, I.b->cols(), bmax, nI, nk, f, ra, ro, (u32*)kb->p, nvr.c);
+    }
+    LAUNCH_COUNT(ctx);
+    TRY(new_values(ctx, os, G.b->col, nvr.c, (u32*)kb->p, ng, &N.b));
+  }
+  // 4. the old outputs at the affected times, negated, merged with the new ones
+  BatchHold O, On;
+  TRY(roll_gather(ctx, out_tr, nk, W.cc(), m, &O.b));
+  if (O.b->n == 0) { *out = N.b; N.b = nullptr; return DBSP_OK; }
+  const u64 no = O.b->n;
+  ROWS32(no, "rolling_aggregate: old outputs");
+  BufP ob;
+  TRY(dev_alloc(ctx, (size_t)(no + 1) * 4 + (size_t)no * 8 + 8, &ob));
+  i64* neww = (i64*)ob->p;
+  u32* keep = (u32*)(neww + no);
+  {
+    ProfScope ps(ctx, KID_ROLLING, no * ((u64)(nk + 1) * 8 + 8 + 8 + 4));
+    k_roll_retract<<<blocks(no + 1), TB, 0, st>>>(O.b->cols(), O.b->w, no, I.b->cols(), bmax, nI, nk, f, keep, neww);
+  }
+  LAUNCH_COUNT(ctx);
+  TRY(compact_ordered(ctx, os, O.b->cols(), neww, keep, no, &On.b));
+  return merge_batches(ctx, N.b, On.b, out);
 }
 
 // Map/FlatMap/Index::eval + from_tuples (operator/filter_map.rs:563-577,700-724)

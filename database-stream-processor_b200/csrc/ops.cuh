@@ -27,6 +27,8 @@ int32_t op_join_batches(Ctx* ctx, const Batch* l, const Batch* r, const F* proj,
 int32_t op_aggregate_delta(Ctx* ctx, const Batch* delta, const Spine* in_tr, const Spine* out_tr, int kind, Batch** out);
 int32_t op_aggregate_fold(Ctx* ctx, const Batch* delta, const Spine* in_tr, const Spine* out_tr, const dbsp_fold* fold,
                           Batch** out);
+int32_t op_rolling_aggregate(Ctx* ctx, const Batch* delta, const Spine* in_tr, const Spine* out_tr,
+                             const dbsp_rel_range& range, int kind, const dbsp_rowfn* f, Batch** out);
 int32_t op_upsert_commands(Ctx* ctx, const dbsp_schema& table, const Cols& in, const uint8_t* insert, u64 n, u64 seq0,
                            Batch** out);
 int32_t op_upsert_delta(Ctx* ctx, const Batch* cmds, const Spine* table, Batch** out);

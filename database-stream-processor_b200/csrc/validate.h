@@ -338,6 +338,66 @@ inline Refusal valid_upsert(const void* out_ptr, const dbsp_schema* cmds, const 
   return {};
 }
 
+// ---- rolling aggregates (dbsp_rolling_aggregate) ---------------------------------------------------------------
+// The output schema of a rolling aggregate over `in`: the partition key's lanes, then TS, the u64 `some` flag and the
+// aggregate's lanes (agg_types, n_agg of them).
+inline dbsp_schema rolling_out_schema(const dbsp_schema& in, const uint8_t* agg_types, int n_agg) {
+  dbsp_schema o;
+  memset(&o, 0, sizeof(o));
+  const int nk = in.n_key_lanes;
+  o.n_key_lanes = (uint8_t)nk;
+  o.n_val_lanes = (uint8_t)(2 + n_agg);
+  for (int l = 0; l < nk; l++) o.lane_types[l] = in.lane_types[l];
+  o.lane_types[nk] = in.lane_types[nk];
+  o.lane_types[nk + 1] = DBSP_U64;
+  for (int l = 0; l < n_agg; l++) o.lane_types[nk + 2 + l] = agg_types[l];
+  return o;
+}
+// rolling_aggregate: the out-pointer and the operands; a kind of the enum; delta and in_trace of one schema with a TS
+// value lane (and a V lane for Max / Min); f for LINEAR only, a row function of value lanes only over KEY, LVAL (V)
+// and CONST whose lanes fit beside PK, TS and `some`; out_trace of exactly rolling_out_schema; a range whose `from`
+// is not after its `to`; and, for an i64 TS, offsets that fit i64.
+inline Refusal valid_rolling(const void* out_ptr, const dbsp_schema* d, const dbsp_schema* i, const dbsp_schema* o,
+                             const dbsp_rel_range* r, int32_t kind, const dbsp_rowfn* f) {
+  const std::string what = "rolling_aggregate";
+  DV_CHECK(not_null(out_ptr, what, "out"));
+  DV_CHECK(not_null(d, what, "delta"));
+  DV_CHECK(not_null(i, what, "in_trace"));
+  DV_CHECK(not_null(o, what, "out_trace"));
+  DV_CHECK(not_null(r, what, "range"));
+  if (kind < DBSP_ROLLING_LINEAR || kind > DBSP_ROLLING_MIN) return what + ": kind = " + std::to_string(kind) + " is not a rolling aggregator";
+  const dbsp_schema &delta = *d, &in = *i;
+  if (!same_schema(delta, in)) return what + ": delta and in_trace differ in schema";
+  const int nk = delta.n_key_lanes, nv = delta.n_val_lanes;
+  if (nv < 1) return what + ": delta has no value lanes; value lane 0 is the timestamp";
+  if (kind != DBSP_ROLLING_LINEAR && nv < 2) return what + ": ROLLING_MAX / ROLLING_MIN need a value lane after the timestamp";
+  if (kind == DBSP_ROLLING_LINEAR && !f) return what + ": f is NULL; ROLLING_LINEAR needs a row function";
+  if (kind != DBSP_ROLLING_LINEAR && f) return what + ": f is given; only ROLLING_LINEAR takes a row function";
+  uint8_t agg_types[DBSP_MAX_LANES];
+  int n_agg = nv - 1;
+  for (int l = 0; l < n_agg; l++) agg_types[l] = delta.lane_types[nk + 1 + l];
+  if (f) {
+    DV_CHECK(valid_rowfn(f, nk, nv - 1, 0, what));
+    const dbsp_schema& fs = f->out_schema;
+    const int room = DBSP_MAX_LANES - nk - 2;
+    if (fs.n_key_lanes != 0 || fs.n_val_lanes < 1 || fs.n_val_lanes > room)
+      return what + ": f.out_schema must have value lanes only, 1.." + num(room > 0 ? room : 0) +
+             " of them (PK, the timestamp and `some` take the other lanes)";
+    n_agg = fs.n_val_lanes;
+    for (int l = 0; l < n_agg; l++) agg_types[l] = fs.lane_types[l];
+  } else if (nk + 2 + n_agg > DBSP_MAX_LANES) {
+    return what + ": PK, the timestamp, `some` and the value lanes need " + num(nk + 2 + n_agg) + " lanes; a row has at most 8";
+  }
+  if (!same_schema(*o, rolling_out_schema(delta, agg_types, n_agg)))
+    return what + ": out_trace must have delta's key lanes, then the timestamp, a u64 `some` lane and the aggregate's lanes";
+  const bool ordered = !r->from_after ? (r->to_after || r->from_off >= r->to_off)
+                                      : (r->to_after ? r->from_off <= r->to_off : (r->from_off == 0 && r->to_off == 0));
+  if (!ordered) return what + ": range.from lies after range.to";
+  if (delta.lane_types[nk] == DBSP_I64 && (r->from_off > (uint64_t)INT64_MAX || r->to_off > (uint64_t)INT64_MAX))
+    return what + ": range offsets of an i64 timestamp must be at most 2^63-1";
+  return {};
+}
+
 // ---- one check per family of calls, in the order of the DESIGN §1 audit ------------------------------------------
 // Closures: a row expression (dbsp_proj) or a row function (dbsp_rowfn, `extra` as for valid_rowfn), and the
 // columns of a raw table each reads.

@@ -1,4 +1,5 @@
-"""Nexmark q0 / q1 / q2 / q3 / q4 / q6 / q7 / q18, and q5 as its SQL states it (q5_hop), on the Stream API.
+"""Nexmark q0 / q1 / q2 / q3 / q4 / q6 / q7 / q18, and q5 as its SQL states it (q5_hop), on the Stream API; and
+`rolling_bids`, a rolling aggregate over the bid stream that no reference query has.
 
 The reference's `NexmarkStream` is one stream of `Event` enum rows
 (crates/nexmark/src/queries/mod.rs:12); here it is three column tables
@@ -9,8 +10,8 @@ from __future__ import annotations
 
 from dataclasses import dataclass
 
-from ..circuit import Fold, Max, Min, RootCircuit, Stream, TableStream
-from ..zset import Proj, Schema, acc, col, const, fanout_index, key, lval, rval
+from ..circuit import Fold, Linear, Max, Min, RootCircuit, Stream, TableStream
+from ..zset import Before, Proj, RelRange, Schema, acc, col, const, fanout_index, key, lval, rval
 
 WATERMARK_INTERVAL_SECONDS = 4  # queries/mod.rs:12
 TUMBLE_SECONDS = 10             # queries/q7.rs:43
@@ -146,6 +147,27 @@ def q18(inp: NexmarkTables) -> Stream:
     bids = inp.bid.flat_map_index(Proj(Schema("uu", "uuuuu"), [col(0), col(1), col(0), col(1), col(2), col(3), col(4)]))
     last = Fold([0] * 5, [key(0), key(1), lval(2), lval(3), lval(4)], where=lval(3).gt(acc(3)))
     return bids.aggregate(last).map(Proj(Schema("uuuuu"), [lval(i) for i in range(5)]))
+
+
+ROLLING_RANGE = RelRange(Before(1000), Before(0))   # the last second of bids, the bid's own millisecond included
+
+
+def rolling_bids(inp: NexmarkTables, watermark: bool = False) -> tuple[Stream, Stream]:
+    """Per auction and bid time, over the auction's bids of the last second (ROLLING_RANGE): (auction, (date_time,
+    some, count, sum of price)) from a Linear aggregate and (auction, (date_time, some, max price)) from Max.
+    watermark=True: the same outputs from partitioned_rolling_aggregate_with_watermark over the bids indexed by
+    date_time, with a watermark WATERMARK_INTERVAL_SECONDS behind the latest bid, so the state stays bounded.
+    Not in QUERIES: the reference's Nexmark suite has no rolling aggregate."""
+    count_sum = Linear(Proj(Schema("", "ii"), [const(1), lval(0)]))
+    if not watermark:
+        by_auction = inp.bid.flat_map_index(Proj(Schema("u", "uu"), [col(0), col(3), col(2)]))   # (auction, (ts, price))
+        return (by_auction.partitioned_rolling_aggregate(count_sum, ROLLING_RANGE),
+                by_auction.partitioned_rolling_aggregate(Max, ROLLING_RANGE))
+    by_time = inp.bid.flat_map_index(Proj(Schema("u", "uu"), [col(3), col(0), col(2)]))          # (ts, (auction, price))
+    wm = by_time.watermark_monotonic(lambda dt: dt - WATERMARK_INTERVAL_SECONDS * 1000)
+    partition = Proj(Schema("u", "u"), [lval(0), lval(1)])                                        # (auction, price)
+    return (by_time.partitioned_rolling_aggregate_with_watermark(wm, partition, count_sum, ROLLING_RANGE),
+            by_time.partitioned_rolling_aggregate_with_watermark(wm, partition, Max, ROLLING_RANGE))
 
 
 QUERIES = {"q0": q0, "q1": q1, "q2": q2, "q3": q3, "q4": q4, "q7": q7, "q5_hop": q5_hop, "q6": q6, "q18": q18}

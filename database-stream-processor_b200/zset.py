@@ -467,6 +467,80 @@ def _factor(f):
     return "weigh_fn", compile_rowfn(Schema("u"), [e])
 
 
+class Before:
+    """RelOffset::Before(n) (time_series/range.rs): n time units before a timestamp."""
+    after = False
+
+    def __init__(self, n: int):
+        if int(n) < 0:
+            raise ValueError(f"{type(self).__name__}({n}): an offset is a non-negative magnitude")
+        self.n = int(n)
+
+    def __neg__(self):
+        return (After if not self.after else Before)(self.n)
+
+    def __eq__(self, o):
+        return type(o) is type(self) and o.n == self.n
+
+    def __repr__(self):
+        return f"{type(self).__name__}({self.n})"
+
+    def add(self, o, signed: bool):
+        """RelOffset + RelOffset (range.rs), saturating in TS's type"""
+        top = (1 << 63) - 1 if signed else (1 << 64) - 1
+        if self.after == o.after:
+            return type(self)(min(self.n + o.n, top))
+        pos, neg = (self, o) if self.after else (o, self)   # After(pos.n) + Before(neg.n)
+        return After(pos.n - neg.n) if pos.n >= neg.n else Before(neg.n - pos.n)
+
+    def sub(self, o, signed: bool):
+        return self.add(-o, signed)
+
+
+class After(Before):
+    """RelOffset::After(n) (time_series/range.rs): n time units after a timestamp."""
+    after = True
+
+
+def _ts_bounds(signed: bool):
+    return (-(1 << 63), (1 << 63) - 1) if signed else (0, (1 << 64) - 1)
+
+
+class RelRange:
+    """RelRange{from, to} (time_series/range.rs) of a rolling aggregate: the range of a timestamp ts is
+    [from(ts), to(ts)], each end Before(n) or After(n).  `frm` is not after `to`."""
+
+    def __init__(self, frm: Before, to: Before):
+        self.frm, self.to = frm, to
+
+    def __repr__(self):
+        return f"RelRange({self.frm!r}, {self.to!r})"
+
+    def c(self) -> capi.CRelRange:
+        r = capi.CRelRange()
+        r.from_after, r.to_after, r.from_off, r.to_off = int(self.frm.after), int(self.to.after), self.frm.n, self.to.n
+        return r
+
+    def range_of(self, ts: int, signed: bool):
+        """(from, to) of timestamp ts, or None when the range lies outside TS's type (range_of: a `from` After is a
+        checked add, a `to` Before a checked subtract, the other ends saturate)"""
+        lo, hi = _ts_bounds(signed)
+        f = ts + self.frm.n if self.frm.after else ts - self.frm.n
+        t = ts + self.to.n if self.to.after else ts - self.to.n
+        if (self.frm.after and f > hi) or (not self.to.after and t < lo):
+            return None
+        return max(lo, min(hi, f)), max(lo, min(hi, t))
+
+    def affected_range_of(self, ts: int, signed: bool):
+        """(from, to) of the timestamps whose range holds ts, or None (affected_range_of)"""
+        lo, hi = _ts_bounds(signed)
+        f = ts - self.to.n if self.to.after else ts + self.to.n
+        t = ts - self.frm.n if self.frm.after else ts + self.frm.n
+        if (not self.to.after and f > hi) or (self.frm.after and t < lo):
+            return None
+        return max(lo, min(hi, f)), max(lo, min(hi, t))
+
+
 class Batch:
     """Owning handle of an immutable device (or oracle) batch."""
 
@@ -993,6 +1067,16 @@ class Backend:
         out = self._out()
         self.api.call("upsert_delta", self.ctx, cmds.h, table.h, C.byref(out))
         return Batch(self, out.value, table.schema)
+
+    def rolling_aggregate(self, delta: Batch, in_trace: Spine, out_trace: Spine, rng: RelRange, kind: int,
+                          f: Proj | None = None) -> Batch:
+        """PartitionedRollingAggregate::eval (dbsp_rolling_aggregate): the change of the rolling aggregate's output
+        at the times `delta` affects.  `f` is LINEAR's row function (a Proj of value lanes only), None otherwise."""
+        out = self._out()
+        fc = None if f is None else C.byref(f._c if f.is_fn else f.as_rowfn()._c)
+        self.api.call("rolling_aggregate", self.ctx, delta.h, in_trace.h, out_trace.h, C.byref(rng.c()), kind, fc,
+                      C.byref(out))
+        return Batch(self, out.value, out_trace.schema)
 
     def weigh(self, b: Batch, f, mode: int) -> Batch:
         """f: a value of the key / value lanes, or a one-lane Proj whose filter drops rows."""

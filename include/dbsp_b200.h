@@ -525,6 +525,42 @@ int32_t dbsp_upsert_commands(dbsp_ctx* ctx, const dbsp_schema* table,
  * gives for the table; its weights are not read. */
 int32_t dbsp_upsert_delta(dbsp_ctx* ctx, const dbsp_batch* cmds,
                           const dbsp_spine* table, dbsp_batch** out);
+/* Relative time range of a rolling aggregate (time_series/range.rs RelRange /
+ * RelOffset).  Each end is Before(off) or After(off), off a magnitude.  For a
+ * timestamp ts, range_of(ts) = [from(ts), to(ts)] in the TS lane's type: a
+ * `from` Before saturates and After is a checked add (overflow: no range); a
+ * `to` Before is a checked subtract (underflow: no range) and After saturates.
+ * affected_range_of(ts), the times whose range holds ts, mirrors it. */
+typedef struct dbsp_rel_range {
+  uint8_t from_after, to_after;   /* 0 = Before(off), 1 = After(off) */
+  uint8_t pad_[6];
+  uint64_t from_off, to_off;      /* magnitudes; i64 TS: at most INT64_MAX */
+} dbsp_rel_range;
+enum dbsp_rolling_kind { DBSP_ROLLING_LINEAR = 0, DBSP_ROLLING_MAX = 1, DBSP_ROLLING_MIN = 2 };
+/* PartitionedRollingAggregate::eval (time_series/rolling_aggregate.rs:436-604).
+ * delta and in_trace have one schema: the key lanes are the partition key PK
+ * (none: one partition), value lane 0 is the timestamp TS and the other value
+ * lanes are V.  For every (pk, ts) with a row of positive weight in in_trace
+ * (weights summed over its batches) and a range_of(ts), the output integral
+ * holds (pk, (ts, some, agg..)) with weight 1, where agg aggregates the rows
+ * (pk, ts', v) of non-zero weight with ts' in range_of(ts):
+ *   LINEAR  per output lane of f(pk, v) (a dbsp_rowfn over KEY, LVAL = V and
+ *           CONST with value lanes only), the sum of f * weight, wrapping;
+ *           a row whose keep flag is 0 adds 0;
+ *   MAX/MIN the lexicographically greatest / least V tuple (max.rs:36-55).
+ * some = 0 (and agg lanes 0) when no row lies in the range.  The call returns
+ * the change of that integral for the times the delta affects (the union of
+ * affected_range_of(d) and [d, d] per delta time d): out_trace's rows there
+ * retracted, the recomputed rows inserted.  out_trace has PK's key lanes and
+ * the value lanes (TS, u64 some, agg lanes): f's lanes or V's.  As with
+ * dbsp_aggregate_delta, the caller has already inserted delta into in_trace
+ * and inserts *out into out_trace afterwards; in_trace need not be delta's
+ * integral (the watermark form feeds it a windowed stream).  `f` is given for
+ * LINEAR and must be NULL otherwise.  A delta of 2^30 or more rows, or 16
+ * trace batches of 2^32-1 or more rows, is DBSP_ERR_UNSUPPORTED. */
+int32_t dbsp_rolling_aggregate(dbsp_ctx* ctx, const dbsp_batch* delta, const dbsp_spine* in_trace,
+                               const dbsp_spine* out_trace, const dbsp_rel_range* range, int32_t kind,
+                               const dbsp_rowfn* f, dbsp_batch** out);
 /* weigh (aggregate/mod.rs:297-323). `f` gives f(k,v) (SRC_KEY/SRC_LVAL).
  * `mode` is a dbsp_weigh_mode; WEIGH_AVG adds a key lane (at most 7 before). */
 int32_t dbsp_weigh(dbsp_ctx* ctx, const dbsp_batch* b, const dbsp_expr* f,

@@ -1,10 +1,12 @@
 // rowfn_oracle.cpp — the CPU oracle with row functions (dbsp_rowfn, include/dbsp_b200.h): the whole oracle of
 // oracle/dbsp_oracle.cpp, unchanged, plus the `_fn` and `_fanout` entry points, dbsp_antijoin_delta,
-// dbsp_aggregate_fold and the set / map input calls (dbsp_upsert_commands, dbsp_upsert_delta), in one translation unit
+// dbsp_aggregate_fold, the set / map input calls (dbsp_upsert_commands, dbsp_upsert_delta) and dbsp_rolling_aggregate, in one translation unit
 // so that they build on its batches, traces, consolidation and error text.  The oracle's own library stays the checker
 // of every `dbsp_proj` test; this one (libdbsp_oracle_fn.so, test infrastructure like it, never linked into the
-// product) is the checker of the row-function, antijoin, fold and upsert tests.  The interpreter below is written apart from the CUDA library's; validate.h is shared,
+// product) is the checker of the row-function, antijoin, fold, upsert and rolling aggregate tests.  The interpreter below is written apart from the CUDA library's; validate.h is shared,
 // so both libraries refuse the same programs with the same texts.
+#include <deque>
+
 #include "../oracle/dbsp_oracle.cpp"
 
 namespace {
@@ -147,9 +149,147 @@ void upsert_key(Builder& bld, const Spine& out_tr, const u64* key, const u64* ne
   }
 }
 
+// range.rs's timestamp arithmetic in the TS lane's type (i64 when sgn), in 128-bit integers: checked forms return
+// false when the result leaves the type, saturating ones clamp to it.
+struct RollTs {
+  bool sgn;
+  __int128 lo() const { return sgn ? (__int128)INT64_MIN : 0; }
+  __int128 hi() const { return sgn ? (__int128)INT64_MAX : (__int128)~0ull; }
+  __int128 val(u64 x) const { return sgn ? (__int128)(i64)x : (__int128)x; }
+  bool fits(__int128 v) const { return v >= lo() && v <= hi(); }
+  u64 clamp(__int128 v) const { return (u64)(v < lo() ? lo() : v > hi() ? hi() : v); }
+  bool lt(u64 a, u64 b) const { return val(a) < val(b); }
+  // RelRange::range_of / affected_range_of
+  bool range_of(const dbsp_rel_range& r, u64 ts, u64* from, u64* to) const {
+    const __int128 t = val(ts);
+    const __int128 f = r.from_after ? t + r.from_off : t - r.from_off, e = r.to_after ? t + r.to_off : t - r.to_off;
+    if ((r.from_after && !fits(f)) || (!r.to_after && !fits(e))) return false;
+    *from = clamp(f);
+    *to = clamp(e);
+    return true;
+  }
+  bool affected_of(const dbsp_rel_range& r, u64 ts, u64* from, u64* to) const {
+    const __int128 t = val(ts);
+    const __int128 f = r.to_after ? t - r.to_off : t + r.to_off, e = r.from_after ? t - r.from_off : t + r.from_off;
+    if ((!r.to_after && !fits(f)) || (r.from_after && !fits(e))) return false;
+    *from = clamp(f);
+    *to = clamp(e);
+    return true;
+  }
+};
+
 }  // namespace
 
 extern "C" {
+
+// PartitionedRollingAggregate::eval (operator/time_series/rolling_aggregate.rs:436-604) as it reads, with the radix
+// tree replaced by a walk of each affected partition in ts order: per partition key of delta, the affected ranges
+// (affected_range_of(d) and [d, d] per delta time, merged), out_trace's rows in them retracted, then the partition's
+// rows of in_trace (weights summed over the batches, zeros skipped) walked once with two window ends that only move
+// forward: running sums for LINEAR, a monotone deque of candidates for MAX / MIN.  Written apart from the CUDA
+// library's gather, prefix sums and sparse table.
+int32_t orc_rolling_aggregate(orc_ctx* c, const orc_batch* delta, const orc_spine* in_tr, const orc_spine* out_tr,
+                              const dbsp_rel_range* range, int32_t kind, const dbsp_rowfn* f, orc_batch** out) {
+  NOT_NULL(c, "ctx");
+  REFUSE(dv::valid_rolling(out, S(delta), S(in_tr), S(out_tr), range, kind, f));
+  const Batch& D = *delta->p;
+  const dbsp_schema& os = out_tr->s.s;
+  const int nk = D.s.n_key_lanes, nvv = D.s.n_val_lanes - 1, n_agg = os.n_val_lanes - 2;
+  const RollTs T{D.s.lane_types[nk] == DBSP_I64};
+  const uint8_t* vty = D.s.lane_types + nk + 1;
+  Tuples t(os);
+  std::vector<std::pair<KV, i64>> grp;
+  u64 row[MAXL], v[MAXL] = {0}, st[DBSP_MAX_STACK];
+  for (size_t k = 0; k < D.K.n; k++) {
+    D.K.get(k, row);
+    // affected ranges, sorted and merged
+    std::vector<std::pair<u64, u64>> iv;
+    size_t lo, hi;
+    D.vrange(k, lo, hi);
+    for (size_t j = lo; j < hi; j++) {
+      const u64 d = D.V.c[0][j];
+      u64 a, b;
+      iv.push_back({d, d});
+      if (T.affected_of(*range, d, &a, &b)) iv.push_back({a, b});
+    }
+    std::sort(iv.begin(), iv.end(), [&](auto& x, auto& y) { return T.lt(x.first, y.first); });
+    std::vector<std::pair<u64, u64>> ranges;
+    for (auto& r : iv) {
+      if (!ranges.empty() && !T.lt(ranges.back().second, r.first)) {
+        if (T.lt(ranges.back().second, r.second)) ranges.back().second = r.second;
+      } else {
+        ranges.push_back(r);
+      }
+    }
+    auto affected = [&](size_t& ri, u64 ts) {   // ts ascending across calls
+      while (ri < ranges.size() && T.lt(ranges[ri].second, ts)) ri++;
+      return ri < ranges.size() && !T.lt(ts, ranges[ri].first);
+    };
+    // retract the old outputs
+    key_group(out_tr->s, row, grp);
+    size_t ri = 0;
+    for (auto& g : grp) {
+      if (g.second == 0) continue;
+      g.first.b->V.get(g.first.pos, row + nk);
+      if (affected(ri, row[nk])) t.push(row, (i64)((u64)0 - (u64)g.second));
+    }
+    // the partition's rows in (ts, v) order
+    key_group(in_tr->s, row, grp);
+    std::vector<u64> ts;
+    std::vector<i64> w;
+    std::vector<std::vector<u64>> vals;
+    for (auto& g : grp) {
+      if (g.second == 0) continue;
+      g.first.b->V.get(g.first.pos, v);
+      ts.push_back(v[0]);
+      w.push_back(g.second);
+      vals.emplace_back(v + 1, v + 1 + nvv);
+    }
+    const size_t n = ts.size();
+    // LINEAR: each row's term f(pk, v) * w; MAX / MIN: rows compared by V
+    std::vector<std::vector<u64>> term(n, std::vector<u64>(std::max(n_agg, 0), 0));
+    if (kind == DBSP_ROLLING_LINEAR)
+      for (size_t j = 0; j < n; j++) {
+        run_rowfn(*f, Env{row, vals[j].data(), vals[j].data()}, st);
+        if (st[n_agg] != 0)
+          for (int l = 0; l < n_agg; l++) term[j][l] = st[l] * (u64)w[j];
+      }
+    const int sign = kind == DBSP_ROLLING_MAX ? 1 : -1;
+    auto not_worse = [&](size_t a, size_t b) {   // row a's V at least as good as row b's
+      return sign * cmp_tuples(vty, nvv, vals[a].data(), vals[b].data()) >= 0;
+    };
+    std::vector<u64> sum(std::max(n_agg, 0), 0);
+    std::deque<size_t> dq;
+    size_t wl = 0, wh = 0;   // the window is rows [wl, wh)
+    ri = 0;
+    for (size_t j = 0; j < n;) {
+      size_t e = j;
+      bool pos = false;
+      for (; e < n && ts[e] == ts[j]; e++) pos = pos || w[e] > 0;
+      u64 from, to;
+      if (pos && affected(ri, ts[j]) && T.range_of(*range, ts[j], &from, &to)) {
+        for (; wh < n && !T.lt(to, ts[wh]); wh++) {
+          for (int l = 0; l < n_agg; l++) sum[l] += term[wh][l];
+          if (kind != DBSP_ROLLING_LINEAR) {
+            while (!dq.empty() && not_worse(wh, dq.back())) dq.pop_back();
+            dq.push_back(wh);
+          }
+        }
+        for (; wl < wh && T.lt(ts[wl], from); wl++)
+          for (int l = 0; l < n_agg; l++) sum[l] -= term[wl][l];
+        while (!dq.empty() && dq.front() < wl) dq.pop_front();
+        row[nk] = ts[j];
+        row[nk + 1] = wl < wh ? 1 : 0;
+        for (int l = 0; l < n_agg; l++)
+          row[nk + 2 + l] = wl >= wh ? 0 : kind == DBSP_ROLLING_LINEAR ? sum[l] : vals[dq.front()][l];
+        t.push(row, 1);
+      }
+      j = e;
+    }
+  }
+  *out = wrap(t.build());
+  return DBSP_OK;
+}
 
 int32_t orc_batch_from_table_fn(orc_ctx* c, const u64* const* cols, uint32_t ncols, const i64* w, u64 n, int32_t,
                                 const dbsp_rowfn* fn, orc_batch** out) {
